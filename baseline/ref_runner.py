@@ -1,6 +1,6 @@
-"""Harness around the UNMODIFIED reference (staged in git-ignored `baseline/_ref/` by
-`baseline/stage_ref.py`) for bench.py's reference arms. Nothing of hero_b200's model, kernels or
-engine is on this path: the reference's own `HierarchicalVlModel` (model/model.py:117-237) and
+"""Harness around the UNMODIFIED reference (staged in the git-ignored `oracle/_ref/` by
+`oracle/stage_ref.py`, which `__graft_entry__.build()` runs) for bench.py's reference arms.
+Nothing of hero_b200's model, kernels or engine is on this path: the reference's own `HierarchicalVlModel` (model/model.py:117-237) and
 `CrossModalTrm` (model/encoder.py:297-352) run through stock PyTorch.
 
 Un-vendored dependencies are replaced by in-memory stand-ins (SURVEY.md Appendix B):
@@ -22,7 +22,7 @@ import types
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF_DIR = os.path.join(HERE, "_ref")
+REF_DIR = os.path.join(os.path.dirname(HERE), "oracle", "_ref")
 
 
 def available():
@@ -30,7 +30,7 @@ def available():
 
 
 def install(dist_backed=False):
-    """Registers the stand-in modules and puts baseline/_ref first on sys.path."""
+    """Registers the stand-in modules and puts oracle/_ref first on sys.path."""
     def mod(name, **attrs):
         m = types.ModuleType(name)
         m.__dict__.update(attrs)

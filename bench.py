@@ -1,5 +1,5 @@
 """Headline benchmark: clips/sec, forward + backward of the HERO hierarchical encoder at
-train-tvr-8gpu shapes (BASELINE.json), data-parallel over N B200s.
+train-tvr-8gpu shapes (BASELINE.json), data-parallel over N H100s.
 
     python bench.py --gpus 1 --steps 20 --warmup 5
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
@@ -25,12 +25,12 @@ same run and reported under `extra`.
           plan's index arrays are copied host->device on a side stream (prefetch one step ahead,
           like the reference's PrefetchLoader, data/loader.py:89-144) and a loss scalar is read
           back. The loader is primed (two plans in flight) when the timed region starts.
-`gpu_reference`  the UNMODIFIED reference modules (staged in git-ignored baseline/_ref by
-          baseline/stage_ref.py; apex FusedLayerNorm -> torch.nn.LayerNorm, Horovod ->
+`gpu_reference`  the UNMODIFIED reference modules (staged in git-ignored oracle/_ref by
+          oracle/stage_ref.py; apex FusedLayerNorm -> torch.nn.LayerNorm, Horovod ->
           torch.distributed shim) doing the same step on the same GPU(s) in the same run under
           torch.autocast(bfloat16): the PyTorch-GPU baseline of BASELINE.json's north star.
 `cpu_baseline` / `--impl reference`  the same reference modules on the host cores (fp32); falls
-          back to the oracle port (kind "port") only if baseline/_ref was not staged.
+          back to the oracle port (kind "port") only if oracle/_ref was not staged.
 """
 import argparse
 import collections
@@ -52,6 +52,22 @@ import torch  # noqa: E402
 
 H, INTER, HEADS, F_LAYERS, C_LAYERS, D = 768, 3072, 12, 6, 3, 4352
 METRIC = "clips/sec fwd+bwd HERO encoder (TVR 8gpu shapes)"
+H100_BF16_DENSE_TFLOPS = 989.0     # NVIDIA H100 SXM data sheet (700 W); a ceiling, not a measurement
+DUMP_GRAD_SAMPLES = 1 << 22        # entries of the flat gradient written by --dump-outputs (16 MB)
+
+
+def dump_outputs(out_dir, clip, q, gflat):
+    """What the timed step returns to its caller, as float32 .npy files: the clip representations,
+    the query-row outputs and a fixed, seeded sample of the flat parameter gradient (the whole
+    buffer is ~0.4 GB)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    g = torch.Generator().manual_seed(0)
+    idx = torch.randint(0, gflat.numel(), (min(DUMP_GRAD_SAMPLES, gflat.numel()),), generator=g)
+    arrays = {"clip": clip, "query": q, "grad_sample": gflat.view(-1)[idx.to(gflat.device)]}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 def model_json(path):
@@ -333,6 +349,7 @@ def run_ours(args):
             if clip_norm is not None:
                 opt.clip_grad_norm_device_(clip_norm)
             opt.step()
+        state["out"] = (clip, q)
         return clip
 
     # ------------------------------------------------------------- device-resident timing
@@ -374,14 +391,15 @@ def run_ours(args):
     ms_total, ms_median, host_enqueue_ms, gaps = timed_loop(resident_step, args.steps, device,
                                                             world, sampler)
     host_free_ms = round(statistics.median(HOST_FREE_MS), 3) if HOST_FREE_MS else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *state["out"], gflat)
     launches = ops.launch_count() // max(args.steps, 1)
     ms_per_step = ms_total / args.steps
     value = world * B / (ms_per_step * 1e-3)
 
     # ------------------------------------------------------------- GEMM-family roofline (live)
     # (the layer runtime keeps everything on one stream while GEMM launches are being timed, so
-    # durations do not overlap). Runs for >= ~2 s so clocks settle where a long job runs, which is
-    # what the "sustained" peak in MEASURED_PEAKS.json was measured under; both fractions reported.
+    # durations do not overlap). Runs for >= ~2 s so clocks settle where a long job runs.
     prof_steps = max(5, min(int(2000.0 / max(ms_per_step * 1.15, 1e-3)), 400))
     if args.roofline_steps > 0:      # profiler runs (ncu launch lists): a short pass is enough
         prof_steps = args.roofline_steps
@@ -397,29 +415,16 @@ def run_ours(args):
         sampler.window(tp0, time.perf_counter())
     gp = ops.stop_gemm_profile()
     profiled_step_ms = p0.elapsed_time(p1) / prof_steps
-    peaks = {}
-    pk_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(pk_path):
-        peaks = json.load(open(pk_path))
-    peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
-    burst_tf = peaks.get("bf16_tflops", 1693.7)
+    peak_tf = H100_BF16_DENSE_TFLOPS
     achieved = gp["flops"] / (gp["ms"] * 1e-3) / 1e12 if gp["ms"] > 0 else 0.0
-    traffic, traffic_src = None, None
-    tr_path = os.path.join(ROOT, "profiles", "gemm_traffic.json")
-    if os.path.exists(tr_path):
-        tj = json.load(open(tr_path))
-        traffic, traffic_src = tj.get("dram_bytes_per_launch"), tj.get("source")
-    roofline = {"bound": "tensor", "kernel": "gemm_tcgen05_kernel (all variants)",
+    roofline = {"bound": "tensor", "kernel": "gemm_wgmma_kernel (all variants)",
                 "achieved": round(achieved, 1), "peak": peak_tf, "unit": "TFLOP/s",
                 "frac": round(achieved / peak_tf, 4),
-                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (of measured); the "
-                               "roofline pass runs >= 2 s" if peaks else
-                               "fallback 1.4 PF/s (of fallback)",
-                "frac_of_burst_peak": round(achieved / burst_tf, 4),
+                "peak_source": "H100 SXM data sheet, dense BF16 at up to 700 W (see 'clocks' "
+                               "for the clocks this run held)",
                 "profiled_steps": prof_steps,
                 "launches_per_step": gp["launches"] // prof_steps,
                 "gemm_share_of_step": round(gp["ms"] / prof_steps / profiled_step_ms, 3),
-                "traffic": traffic, "traffic_source": traffic_src,
                 "step_algorithmic_tflops": round(3 * flops_fwd * 1e-12, 4),
                 "step_frac_of_peak": round(3 * flops_fwd / (ms_per_step * 1e-3) / 1e12 / peak_tf,
                                            4)}
@@ -690,7 +695,7 @@ def run_ours(args):
                        "e2e_batch": "packed (no f_v_feats: frame slots read from c_v_feats through "
                                     "the plan)" if slim else "legacy dict incl. f_v_feats",
                        "l2": "no explicit flush: per-step working set (~0.35 GB weights+grads, "
-                             "~3 GB activations, 56-112 MB inputs) exceeds the 126 MB L2"},
+                             "~3 GB activations, 56-112 MB inputs) exceeds the 50 MB L2"},
             "clocks": clocks, "gpu_launches": launches,
             "host_enqueue_ms_per_step": round(host_enqueue_ms, 3),
             "host_enqueue_ms_queue_not_full": host_free_ms,
@@ -726,14 +731,13 @@ def _ref_inputs(sample_clips, seed=1234):
 
 
 def gpu_reference(args, rank, world, device, B):
-    """The unmodified reference (baseline/_ref) doing the same step on the GPU under
+    """The unmodified reference (oracle/_ref) doing the same step on the GPU under
     torch.autocast(bfloat16): fwd `forward_repr` + `f_encoder('txt')`, backward, and at N > 1 its
     own all_reduce_and_rescale_tensors over a torch.distributed-backed Horovod shim."""
     from baseline import ref_runner as rr
     from hero_b200 import synth
     if rr.available() is None:
-        return {"unavailable": "baseline/_ref not staged (run baseline/stage_ref.py where "
-                               "/root/reference exists)"}
+        return {"unavailable": "oracle/_ref not staged (oracle/stage_ref.py found no reference checkout)"}
     try:
         rr.install(dist_backed=world > 1)
         model = rr.build_model(device, seed=0, train=True)
@@ -786,7 +790,7 @@ def _pick_cpu_threads():
 
 
 def cpu_baseline(sample_clips=8, steps=2, warmup=1):
-    """The reference's own CPU path (unmodified modules from baseline/_ref; oracle port if the
+    """The reference's own CPU path (unmodified modules from oracle/_ref; oracle port if the
     reference was not staged) on all host cores: fwd+bwd on a bounded sample of the same workload
     (first `sample_clips` clips of SYN-TVR-dense)."""
     from baseline import ref_runner as rr
@@ -803,7 +807,7 @@ def cpu_baseline(sample_clips=8, steps=2, warmup=1):
 
         def step():
             ref_step(vb, qb, dclip, dq)
-        what = "unmodified reference modules (baseline/_ref), fp32, torch CPU autograd"
+        what = "unmodified reference modules (oracle/_ref), fp32, torch CPU autograd"
     else:
         from oracle import hero_oracle as orc
         kind = "port"
@@ -892,8 +896,8 @@ def main():
                     help="e2e ships the legacy batch dict including f_v_feats (2x the H2D bytes)")
     ap.add_argument("--grad-zero", default="sync", choices=("async", "sync"),
                     help="zero the flat gradient buffer in the compute stream before the forward "
-                         "(default) or on a side stream beside it (measured equal on B200: the "
-                         "memset's CTAs delay the persistent GEMMs by what they save)")
+                         "(default) or on a side stream beside it (the memset's CTAs compete with "
+                         "the persistent GEMMs)")
     ap.add_argument("--no-extra", action="store_true", help="skip the config-2 / config-3 lines")
     ap.add_argument("--roofline-steps", type=int, default=0,
                     help="steps of the per-launch GEMM timing pass (0 = as many as fill ~2 s)")
@@ -901,6 +905,9 @@ def main():
     ap.add_argument("--no-gpu-reference", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-clips", type=int, default=8)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's outputs (clip, query "
+                         "rows, a seeded sample of the parameter gradient) as float32 DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

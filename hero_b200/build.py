@@ -1,8 +1,8 @@
-"""In-tree build of the C-ABI shared library (nvcc, sm_100a only).
+"""In-tree build of the C-ABI shared library (nvcc, sm_90a only).
 
 `python -m hero_b200.build` compiles every `csrc/*.cu` into `hero_b200/libhero_b200.so`.
-nvcc cross-compiles without a GPU, so this runs on the CPU-only dev box; the resulting `.so`
-is git-ignored but travels to the GPU box with the repo snapshot.
+nvcc cross-compiles without a GPU, so this also runs on a machine without one; the resulting
+`.so` and the object files under `hero_b200/build/` are git-ignored.
 """
 import hashlib
 import os
@@ -17,7 +17,7 @@ BUILD_DIR = os.path.join(PKG_DIR, "build")
 LIB_PATH = os.path.join(PKG_DIR, "libhero_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",

@@ -1,4 +1,4 @@
-// Variable-length multi-head self-attention on the 5th-gen tensor cores (tcgen05 / TMEM / TMA).
+// Variable-length multi-head self-attention on the Hopper tensor cores (wgmma / TMA).
 //
 // HERO's sequences are short (cross-modal rows ~10-70 tokens, temporal rows <= 100 frames), so a
 // 128-row MMA tile would be mostly empty if it held one sequence. Instead the host packs
@@ -10,9 +10,9 @@
 //             layout) -> P (bf16, smem) -> O = P V (128x64x128) -> ctx
 //   backward  S = Q K^T, dP = dO V^T -> P, dS rows -> dV = P^T dO, dK = dS^T Q, dQ = dS K
 //
-// Q/K/V/dO tiles arrive by TMA (128-byte swizzle); every contraction is a tcgen05.mma with fp32
-// accumulators in TMEM. The transposed operands (P^T, dS^T, V/dO/Q/K as [k][n]) need no copies:
-// the SAME smem tiles are addressed as MN-major operands through the UMMA descriptors.
+// Q/K/V/dO tiles arrive by TMA (128-byte swizzle); every contraction is a warpgroup wgmma with
+// fp32 accumulators in registers. The transposed operands (P^T, dS^T, V/dO/Q/K as [k][n]) need no
+// copies: the SAME smem tiles are addressed as MN-major operands through the wgmma descriptors.
 // Softmax statistics, exp2, dropout masks and the P / dS tiles never touch HBM.
 //
 // Replaces model/layers.py:129-160 (BertSelfAttention after the QKV projections) and its autograd
@@ -93,39 +93,25 @@ struct AttnTcArgs {
   float drop_scale;
 };
 
-// Each thread parks its 64-feature row (two 32-column TMEM fragments, optionally scaled) in a
-// swizzled [128 x 128 B] smem tile ...
-__device__ __forceinline__ void stage_row(uint8_t* tile, int row, const uint32_t (&r0)[32],
-                                          const uint32_t (&r1)[32], float scale) {
+// A warp's part of a [64 x 64] wgmma result (rows 16w + l/4 and + 8, columns 8j + 2(l%4) + {0,1}),
+// optionally scaled, parked as bf16 in a swizzled [128 x 128 B] smem tile at tile row row0 + ...
+__device__ __forceinline__ void stage_frag64(uint8_t* tile, int row0, const float (&o)[32],
+                                             float sa, float sb) {
+  const int lane = threadIdx.x & 31;
+  const int fc = (lane & 3) * 2;
 #pragma unroll
-  for (int g = 0; g < 8; ++g) {
-    const uint32_t* r = g < 4 ? r0 : r1;
-    const int b = (g & 3) * 8;
-    uint4 v;
-    v.x = pack_bf16x2(__uint_as_float(r[b]) * scale, __uint_as_float(r[b + 1]) * scale);
-    v.y = pack_bf16x2(__uint_as_float(r[b + 2]) * scale, __uint_as_float(r[b + 3]) * scale);
-    v.z = pack_bf16x2(__uint_as_float(r[b + 4]) * scale, __uint_as_float(r[b + 5]) * scale);
-    v.w = pack_bf16x2(__uint_as_float(r[b + 6]) * scale, __uint_as_float(r[b + 7]) * scale);
-    *reinterpret_cast<uint4*>(tile + row * 128 + ((g ^ (row & 7)) << 4)) = v;
-  }
-}
-// 32 of the row's 64 features (one TMEM fragment): units 4 * half .. 4 * half + 3
-__device__ __forceinline__ void stage_half_row(uint8_t* tile, int row, int half,
-                                               const uint32_t (&r)[32], float scale) {
+  for (int h = 0; h < 2; ++h) {
+    const int r = row0 + (lane >> 2) + 8 * h;
+    const float sc = h ? sb : sa;
 #pragma unroll
-  for (int g = 0; g < 4; ++g) {
-    const int b = g * 8;
-    uint4 v;
-    v.x = pack_bf16x2(__uint_as_float(r[b]) * scale, __uint_as_float(r[b + 1]) * scale);
-    v.y = pack_bf16x2(__uint_as_float(r[b + 2]) * scale, __uint_as_float(r[b + 3]) * scale);
-    v.z = pack_bf16x2(__uint_as_float(r[b + 4]) * scale, __uint_as_float(r[b + 5]) * scale);
-    v.w = pack_bf16x2(__uint_as_float(r[b + 6]) * scale, __uint_as_float(r[b + 7]) * scale);
-    *reinterpret_cast<uint4*>(tile + row * 128 + (((half * 4 + g) ^ (row & 7)) << 4)) = v;
+    for (int j = 0; j < 8; ++j)
+      *reinterpret_cast<uint32_t*>(tile + r * 128 + ((j ^ (r & 7)) << 4) + fc * 2) =
+          pack_bf16x2(o[4 * j + 2 * h] * sc, o[4 * j + 2 * h + 1] * sc);
   }
 }
 // ... and the CTA then writes the tile(s) out with every warp covering 4 full 128-byte rows per
-// instruction (a lane-per-row store would touch 32 different lines per instruction and choked the
-// LSU: `lg_throttle` was the top stall of the first version). Rows >= ntok belong to the next tile.
+// instruction (a lane-per-row store would touch 32 different lines per instruction).
+// Rows >= ntok belong to the next tile.
 __device__ __forceinline__ void store_tiles(const uint8_t* tiles, int n_parts, __nv_bfloat16* base,
                                             long long row_stride, long long part_stride, int ntok) {
   for (int idx = threadIdx.x; idx < n_parts * AT_ROWS * 8; idx += blockDim.x) {
@@ -138,47 +124,51 @@ __device__ __forceinline__ void store_tiles(const uint8_t* tiles, int n_parts, _
   }
 }
 
+// S[64 rows from row 64 * g, 128 keys] of the tile = Q K^T + 16384 * [same sequence], issued by one
+// warpgroup (Q, K K-major; the membership operand MN-major on both sides)
+__device__ __forceinline__ void issue_scores(float (&s)[64], const uint8_t* sQ, const uint8_t* sK,
+                                             const uint8_t* sE, int g) {
+#pragma unroll
+  for (int k = 0; k < AT_D / 16; ++k)
+    wgmma_m64n128k16<0, 0>(s, make_sw128_desc(smem_u32(sQ) + g * 8192 + k * 32, 16, 1024),
+                           make_sw128_desc(smem_u32(sK) + k * 32, 16, 1024), k > 0 ? 1u : 0u);
+  wgmma_m64n128k16<1, 1>(s, make_sw128_desc(smem_u32(sE) + g * 2048, AT_MAX_SEQS * 128, 1024),
+                         make_sw128_desc(smem_u32(sE), AT_MAX_SEQS * 128, 1024), 1u);
+}
+
 // ------------------------------------------------------------------------------------ forward
+// One warpgroup; the 128 query rows are taken as two 64-row halves (S of a half: 64 fp32 registers
+// per thread). The softmax runs on the accumulator fragment: a row's 128 scores are spread over
+// the four lanes of a quad (32 each), so its max and sum take two shuffles.
 __global__ void __launch_bounds__(128)
 attn_tc_fwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnTcArgs a,
                    __nv_bfloat16* __restrict__ ctx, float* __restrict__ lse) {
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0u) __trap();
-  // 48 KB of operand tiles; P (32 KB) is written over Q|K once S = QK^T has retired, and O reuses
-  // S's TMEM columns, so 4 CTAs fit per SM (smem 49 KB, 128 TMEM columns each) and their TMA /
-  // MMA / softmax phases overlap.
+  // Q, K, V operand tiles, then P (32 KB, two 64-column chunks); the output is staged over Q
   uint8_t* sQ = smem;
   uint8_t* sK = smem + AT_TILE_BYTES;
   uint8_t* sV = smem + 2 * AT_TILE_BYTES;
-  uint8_t* sP = smem;
-  uint8_t* sE = smem + 3 * AT_TILE_BYTES;           // sequence-membership operand (4 KB)
+  uint8_t* sP = smem + 3 * AT_TILE_BYTES;
+  uint8_t* sE = sP + AT_P_BYTES;                    // sequence-membership operand (4 KB)
   uint64_t* bars = reinterpret_cast<uint64_t*>(sE + AT_MASK_BYTES);
   uint64_t* tma_bar = bars;
-  uint64_t* mma_bar = bars + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
   int* warp_starts = reinterpret_cast<int*>(bars + 3);
 
   const int tile = blockIdx.x, head = blockIdx.y;
-  const int warp = threadIdx.x >> 5;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tok0 = a.tile_tok0[tile];
   const int ntok = a.tile_ntok[tile];
   // (the plan arrays were uploaded long before the previous kernel started: safe before pdl_wait)
   const int i = threadIdx.x;
   const bool valid = i < ntok;
-  int lo = 0, hi = 0;
-  if (valid) {
-    lo = a.seq_lo[tok0 + i] - tok0;
-    hi = a.seq_hi[tok0 + i] - tok0;
-  }
+  int lo = 0;
+  if (valid) lo = a.seq_lo[tok0 + i] - tok0;
   const uint32_t starts = seq_starts_ballot(valid, lo, i, warp_starts);
 
-  // The tile loads go out first: they need neither TMEM nor the other threads, and the wait for
-  // them was the top stall of the kernel (ncu: 23 % of the samples on this barrier's spin loop)
-  // while TMEM allocation and the membership writes sat in front of their issue.
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_qkv);
     mbar_init(tma_bar, 1);
-    mbar_init(mma_bar, 1);
     fence_barrier_init();
     pdl_wait();
     mbar_arrive_expect_tx(tma_bar, 3 * AT_TILE_BYTES);
@@ -186,15 +176,7 @@ attn_tc_fwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnTcArg
     tma_load_2d(sK, &tmap_qkv, tma_bar, a.H + head * AT_D, tok0);
     tma_load_2d(sV, &tmap_qkv, tma_bar, 2 * a.H + head * AT_D, tok0);
   }
-  __syncwarp();
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, 128);
-    tmem_relinquish();
-  }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
   pdl_wait();
   pdl_launch_dependents();
 
@@ -207,128 +189,79 @@ attn_tc_fwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnTcArg
   __syncthreads();
   mbar_wait(tma_bar, 0);
 
-  if (threadIdx.x == 0) {
-    tc_fence_after_sync();
-    constexpr uint32_t idesc = make_idesc_bf16(128, 128, 0, 0);
-#pragma unroll
-    for (int k = 0; k < AT_D / 16; ++k) {
-      const uint64_t ad = make_sw128_desc(smem_u32(sQ) + k * 32, 16, 1024);
-      const uint64_t bd = make_sw128_desc(smem_u32(sK) + k * 32, 16, 1024);
-      umma_f16(tmem, ad, bd, idesc, k > 0 ? 1u : 0u);
-    }
-    // + 16384 where query and key token belong to the same sequence (E E^T, both MN-major)
-    const uint64_t ed = make_sw128_desc(smem_u32(sE), AT_MAX_SEQS * 128, 1024);
-    umma_f16(tmem, ed, ed, make_idesc_bf16(128, 128, 1, 1), 1u);
-    umma_commit(mma_bar);
-  }
-  mbar_wait(mma_bar, 0);
-  tc_fence_after_sync();
-
-  // ---- softmax on this thread's row: the other sequences' columns underflow to exactly 0 ----
-  // warp-uniform column range (tcgen05.ld is warp-collective)
-  int wlo = valid ? lo : AT_ROWS, whi = hi;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    wlo = min(wlo, __shfl_xor_sync(0xffffffffu, wlo, o));
-    whi = max(whi, __shfl_xor_sync(0xffffffffu, whi, o));
-  }
-  const uint32_t t_row = tmem + (static_cast<uint32_t>(warp * 32) << 16);
-  float mx = -INFINITY;
-  for (int c = 0; c < 4; ++c) {
-    if (c * 32 >= whi || c * 32 + 32 <= wlo) continue;   // warp-uniform
-    uint32_t r[32];
-    tmem_ld_32x32(t_row + c * 32, r);
-    tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 32; ++j) mx = fmaxf(mx, __uint_as_float(r[j]));
-  }
-  const float nmx = -mx * a.scale_log2;
-  float sum0 = 0.f, sum1 = 0.f;
+  const int fc = (lane & 3) * 2;
   const uint32_t k2 = attn_drop_k2(a.drop_thr);
-  for (int c = 0; c < 4; ++c) {
-    uint32_t pk[16];
-    const bool touch = !(c * 32 >= whi || c * 32 + 32 <= wlo);   // warp-uniform
-    if (touch) {
-      uint32_t r[32];
-      tmem_ld_32x32(t_row + c * 32, r);
-      tmem_ld_wait();
+  float inv[2][2];
+#pragma unroll 1
+  for (int g = 0; g < 2; ++g) {
+    float s[64];
+    wgmma_fence();
+    issue_scores(s, sQ, sK, sE, g);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(s);
+    // ---- softmax of rows r[0], r[1]: the other sequences' columns underflow to exactly 0 ----
+    float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-      for (int j = 0; j < 32; j += 2) {
-        const float p0 = ex2(fmaf(__uint_as_float(r[j]), a.scale_log2, nmx));
-        const float p1 = ex2(fmaf(__uint_as_float(r[j + 1]), a.scale_log2, nmx));
-        sum0 += p0;
-        sum1 += p1;
-        pk[j >> 1] = pack_bf16x2(p0, p1);
-      }
-      if (a.drop_thr != 0u) {     // the 1 / (1 - p) scale is folded into the output row scale
+    for (int j = 0; j < 16; ++j)
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const uint32_t h0 = attn_drop_group(a.drop_key, tok0 + i, a.heads, head, c * 4 + g);
+      for (int h = 0; h < 2; ++h) mx[h] = fmaxf(mx[h], fmaxf(s[4 * j + 2 * h], s[4 * j + 2 * h + 1]));
 #pragma unroll
-          for (int k = 0; k < 4; ++k) pk[g * 4 + k] &= attn_keep_mask2(attn_drop_pair(h0, k), k2);
-        }
-      }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 16; ++j) pk[j] = 0u;
+    for (int h = 0; h < 2; ++h) {
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
     }
-    // 32 columns = 4 units of 16 B inside 64-column chunk (c >> 1), units (c & 1) * 4 + g
+    float sum[2] = {0.f, 0.f};
 #pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      const uint4 v = make_uint4(pk[4 * g], pk[4 * g + 1], pk[4 * g + 2], pk[4 * g + 3]);
-      *reinterpret_cast<uint4*>(sP + p_unit_offset(i, c >> 1, (c & 1) * 4 + g)) = v;
+    for (int h = 0; h < 2; ++h) {
+      const int r = g * 64 + warp * 16 + (lane >> 2) + 8 * h;
+      const float nmx = -mx[h] * a.scale_log2;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const float p0 = ex2(fmaf(s[4 * j + 2 * h], a.scale_log2, nmx));
+        const float p1 = ex2(fmaf(s[4 * j + 2 * h + 1], a.scale_log2, nmx));
+        sum[h] += p0 + p1;
+        uint32_t pk = pack_bf16x2(p0, p1);
+        if (a.drop_thr != 0u)      // the 1 / (1 - p) scale is folded into the output row scale
+          pk &= attn_keep_mask2(
+              attn_drop_pair(attn_drop_group(a.drop_key, tok0 + r, a.heads, head, j), fc >> 1), k2);
+        *reinterpret_cast<uint32_t*>(sP + p_unit_offset(r, j >> 3, j & 7) + fc * 2) = pk;
+      }
+      sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 1);
+      sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 2);
+      inv[g][h] = (sum[h] > 0.f ? 1.0f / sum[h] : 0.f) * (a.drop_thr != 0u ? a.drop_scale : 1.0f);
+      if (r < ntok && lse != nullptr && (lane & 3) == 0)   // log2-domain log-sum-exp, for the backward
+        lse[(long long)(tok0 + r) * a.heads + head] = (mx[h] - AT_MASK_BIG) * a.scale_log2 + log2f(sum[h]);
     }
   }
-  const float sum = sum0 + sum1;
   fence_proxy_async();
-  tc_fence_before_sync();
   __syncthreads();
 
-  if (threadIdx.x == 0) {
-    tc_fence_after_sync();
-    constexpr uint32_t idesc = make_idesc_bf16(128, 64, 0, 1);   // A = P (K-major), B = V (MN-major)
+  // O = P V (A = P K-major, B = V MN-major), staged over the dead Q tile
+#pragma unroll 1
+  for (int g = 0; g < 2; ++g) {
+    float o[32];
+    wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < AT_ROWS / 16; ++k) {
-      const uint64_t ad =
-          make_sw128_desc(smem_u32(sP) + (k >> 2) * (AT_ROWS * 128) + (k & 3) * 32, 16, 1024);
-      const uint64_t bd = make_sw128_desc(smem_u32(sV) + k * 2048, AT_TILE_BYTES, 1024);
-      umma_f16(tmem, ad, bd, idesc, k > 0 ? 1u : 0u);   // O overwrites S's columns [0, 64)
-    }
-    umma_commit(mma_bar);
-  }
-  mbar_wait(mma_bar, 1);
-  tc_fence_after_sync();
-
-  {
-    const float inv = (sum > 0.f ? 1.0f / sum : 0.f) * (a.drop_thr != 0u ? a.drop_scale : 1.0f);
-    uint32_t r0[32], r1[32];
-    tmem_ld_32x32(t_row, r0);
-    tmem_ld_32x32(t_row + 32, r1);
-    tmem_ld_wait();
-    if (valid && lse != nullptr)   // log2-domain log-sum-exp of the scaled scores, for the backward
-      lse[(long long)(tok0 + i) * a.heads + head] = (mx - AT_MASK_BIG) * a.scale_log2 + log2f(sum);
-    stage_row(sQ, i, r0, r1, inv);   // Q's tile is dead: P.V has retired
+    for (int k = 0; k < AT_ROWS / 16; ++k)
+      wgmma_m64n64k16<0, 1>(
+          o, make_sw128_desc(smem_u32(sP) + (k >> 2) * (AT_ROWS * 128) + g * 8192 + (k & 3) * 32, 16, 1024),
+          make_sw128_desc(smem_u32(sV) + k * 2048, AT_TILE_BYTES, 1024), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(o);
+    stage_frag64(sQ, g * 64 + warp * 16, o, inv[g][0], inv[g][1]);
   }
   __syncthreads();
   store_tiles(sQ, 1, ctx + (long long)tok0 * a.H + head * AT_D, a.H, 0, ntok);
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem, 128);
-  }
 }
 
 // ------------------------------------------------------------------------------------ backward
-// TMEM (256 columns): S [0,128) and dP [128,256); once every thread has turned them into P / dS,
-// dQ [0,64), dK [64,128), dV [128,192) reuse the same columns. smem (112 KB): Q, K, V, dO tiles;
-// P's first 64-column chunk is written over V (dead after dP = dO V^T), so two CTAs fit per SM and
-// overlap each other's TMA / MMA / softmax phases. Probabilities are rebuilt from the forward's
-// log-sum-exp in ONE pass over S.
-// 256 threads: TWO threads per tile row (warps w and w + 4 share TMEM lane quadrant w), each owning
-// 64 of the row's 128 score columns and 32 of the 64 features of every output row. With only two
-// CTAs per SM (TMEM: 2 x 256 columns) the 128-thread version left the SM with 8 warps to hide the
-// TMEM / MUFU / smem latencies of its longest phase.
+// Two warpgroups; warpgroup g owns tile rows [64g, 64g + 64) of every product. S and dP of its
+// rows stay in registers (2 x 64 per thread) and become P / dS in smem in ONE pass, the
+// probabilities rebuilt from the forward's log-sum-exp. smem (112 KB): Q, K, V, dO tiles;
+// P's first 64-column chunk is written over V, its second over the forward output O (both dead
+// once every S / dP MMA has retired), dS after them.
 constexpr int AT_BWD_THREADS = 256;
 __global__ void __launch_bounds__(AT_BWD_THREADS)
 attn_tc_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
@@ -348,32 +281,26 @@ attn_tc_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
   uint8_t* sdS = smem + 5 * AT_TILE_BYTES;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sdS + AT_P_BYTES);
   uint64_t* tma_bar = bars;
-  uint64_t* mma_bar = bars + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
   int* warp_starts = reinterpret_cast<int*>(bars + 3);
+  float* sDi = reinterpret_cast<float*>(bars + 8);   // D_i of the tile's rows
   uint8_t* sE = sdS;     // membership operand of the S MMA; dS is written after that MMA retired
 
   const int tile = blockIdx.x, head = blockIdx.y;
-  const int warp = threadIdx.x >> 5;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tok0 = a.tile_tok0[tile];
   const int ntok = a.tile_ntok[tile];
-  const int i = threadIdx.x & 127;        // tile row
-  const int half = threadIdx.x >> 7;      // which 64 score columns / 32 output features
+  const int i = threadIdx.x & 127;        // tile row (membership, D_i)
+  const int half = threadIdx.x >> 7;      // = the warpgroup
   const bool valid = i < ntok;
-  int lo = 0, hi = 0;
-  if (valid) {
-    lo = a.seq_lo[tok0 + i] - tok0;
-    hi = a.seq_hi[tok0 + i] - tok0;
-  }
+  int lo = 0;
+  if (valid) lo = a.seq_lo[tok0 + i] - tok0;
   const uint32_t starts = seq_starts_ballot(valid, lo, i, warp_starts);
 
-  // tile loads first (see the forward kernel)
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_qkv);
     tma_prefetch_desc(&tmap_do);
     tma_prefetch_desc(&tmap_o);
     mbar_init(tma_bar, 1);
-    mbar_init(mma_bar, 1);
     fence_barrier_init();
     pdl_wait();
     mbar_arrive_expect_tx(tma_bar, 5 * AT_TILE_BYTES);
@@ -381,22 +308,12 @@ attn_tc_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
     tma_load_2d(sK, &tmap_qkv, tma_bar, a.H + head * AT_D, tok0);
     tma_load_2d(sV, &tmap_qkv, tma_bar, 2 * a.H + head * AT_D, tok0);
     tma_load_2d(sdO, &tmap_do, tma_bar, head * AT_D, tok0);
-    // the forward output O lands where P's second chunk will be written later; every thread has
-    // read its O row before the CTA barrier that precedes the first MMA
+    // the forward output O lands where P's second chunk will be written later
     tma_load_2d(sP + P_CHUNK, &tmap_o, tma_bar, head * AT_D, tok0);
   }
-  __syncwarp();
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, 256);
-    tmem_relinquish();
-  }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
   pdl_wait();
   pdl_launch_dependents();
-
 
   {
     const int ord = seq_ordinal(valid, starts, warp_starts);
@@ -407,214 +324,155 @@ attn_tc_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
   }
   __syncthreads();
   mbar_wait(tma_bar, 0);
-  // S, dP go first; D_i is computed while they run
-  if (threadIdx.x == 0) {
-    tc_fence_after_sync();
-    constexpr uint32_t idesc = make_idesc_bf16(128, 128, 0, 0);
+  // S = Q K^T (+ membership), dP = dO V^T go first; D_i is computed while they run
+  float s[64], dp[64];
+  wgmma_fence();
+  issue_scores(s, sQ, sK, sE, half);
 #pragma unroll
-    for (int k = 0; k < AT_D / 16; ++k) {   // S = Q K^T
-      const uint64_t ad = make_sw128_desc(smem_u32(sQ) + k * 32, 16, 1024);
-      const uint64_t bd = make_sw128_desc(smem_u32(sK) + k * 32, 16, 1024);
-      umma_f16(tmem, ad, bd, idesc, k > 0 ? 1u : 0u);
-    }
-    {   // + 16384 on same-sequence pairs (see AT_MASK_BIG)
-      const uint64_t ed = make_sw128_desc(smem_u32(sE), AT_MAX_SEQS * 128, 1024);
-      umma_f16(tmem, ed, ed, make_idesc_bf16(128, 128, 1, 1), 1u);
-    }
-#pragma unroll
-    for (int k = 0; k < AT_D / 16; ++k) {   // dP = dO V^T
-      const uint64_t ad = make_sw128_desc(smem_u32(sdO) + k * 32, 16, 1024);
-      const uint64_t bd = make_sw128_desc(smem_u32(sV) + k * 32, 16, 1024);
-      umma_f16(tmem + 128, ad, bd, idesc, k > 0 ? 1u : 0u);
-    }
-    umma_commit(mma_bar);
-  }
+  for (int k = 0; k < AT_D / 16; ++k)
+    wgmma_m64n128k16<0, 0>(dp, make_sw128_desc(smem_u32(sdO) + half * 8192 + k * 32, 16, 1024),
+                           make_sw128_desc(smem_u32(sV) + k * 32, 16, 1024), k > 0 ? 1u : 0u);
+  wgmma_commit();
   // D_i = dO_i . O_i from the swizzled smem tiles (conflict-free 16-byte reads)
-  float Di = 0.f;
-  if (valid) {
+  if (half == 0) {
+    float Di = 0.f;
+    if (valid) {
 #pragma unroll
-    for (int g = 0; g < 8; ++g) {
-      const uint32_t off = i * 128 + ((g ^ (i & 7)) << 4);
-      const uint4 o = *reinterpret_cast<const uint4*>(sP + P_CHUNK + off);
-      const uint4 d = *reinterpret_cast<const uint4*>(sdO + off);
-      const uint32_t ow[4] = {o.x, o.y, o.z, o.w}, dw[4] = {d.x, d.y, d.z, d.w};
+      for (int g = 0; g < 8; ++g) {
+        const uint32_t off = i * 128 + ((g ^ (i & 7)) << 4);
+        const uint4 o = *reinterpret_cast<const uint4*>(sP + P_CHUNK + off);
+        const uint4 d = *reinterpret_cast<const uint4*>(sdO + off);
+        const uint32_t ow[4] = {o.x, o.y, o.z, o.w}, dw[4] = {d.x, d.y, d.z, d.w};
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 x = unpack_bf16x2(ow[j]), y = unpack_bf16x2(dw[j]);
-        Di = fmaf(x.x, y.x, Di);
-        Di = fmaf(x.y, y.y, Di);
+        for (int j = 0; j < 4; ++j) {
+          const float2 x = unpack_bf16x2(ow[j]), y = unpack_bf16x2(dw[j]);
+          Di = fmaf(x.x, y.x, Di);
+          Di = fmaf(x.y, y.y, Di);
+        }
       }
     }
+    sDi[i] = Di;
   }
-
-  // both threads of a row have read its O row: its smem is P's second chunk from here on
+  wgmma_wait<0>();
+  wgmma_fence_acc(s);
+  wgmma_fence_acc(dp);
+  // every S / dP MMA has retired and every O row has been read: V, O and E are dead from here on
   __syncthreads();
-  mbar_wait(mma_bar, 0);
-  tc_fence_after_sync();
 
-  int wlo = valid ? lo : AT_ROWS, whi = hi;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    wlo = min(wlo, __shfl_xor_sync(0xffffffffu, wlo, o));
-    whi = max(whi, __shfl_xor_sync(0xffffffffu, whi, o));
-  }
-  const uint32_t t_row = tmem + (static_cast<uint32_t>((warp & 3) * 32) << 16);
-  // exponent offset of this row: its log-sum-exp plus the membership shift; rows past the tile's
-  // end get +inf so that their P and dS rows (which the transposed products sum over) are 0
-  const float row_c = valid ? fmaf(AT_MASK_BIG, a.scale_log2,
-                                   lse[(long long)(tok0 + i) * a.heads + head])
-                            : INFINITY;
   const bool drop = a.drop_thr != 0u;
   const float keep_scale = drop ? a.drop_scale : 1.0f;
   const uint32_t ks_bits = __float_as_uint(keep_scale);
   const uint32_t k2 = attn_drop_k2(a.drop_thr);
+  const int fc = (lane & 3) * 2;
+  const int wrow0 = half * 64 + (warp & 3) * 16;   // this warp's 16 rows
   // Stored tiles: P = bf16(p) on kept lanes (dV = keep_scale * P^T dO, scaled when dV is staged),
   // dS = p * (dP * keep - D) (dQ, dK scaled by 1 / sqrt(d) when staged; a power of two).
-  for (int c = 2 * half; c < 2 * half + 2; ++c) {
-    uint32_t pk[16], dk[16];
-    const bool touch = !(c * 32 >= whi || c * 32 + 32 <= wlo);
-    if (touch) {
-      uint32_t r[32], d[32];
-      tmem_ld_32x32(t_row + c * 32, r);
-      tmem_ld_32x32(t_row + 128 + c * 32, d);
-      tmem_ld_wait();
 #pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        uint32_t h0 = 0u;
-        if (drop) h0 = attn_drop_group(a.drop_key, tok0 + i, a.heads, head, c * 4 + g);
+  for (int h = 0; h < 2; ++h) {
+    const int r = wrow0 + (lane >> 2) + 8 * h;
+    const bool rv = r < ntok;
+    // exponent offset of this row: its log-sum-exp plus the membership shift; rows past the
+    // tile's end get +inf so that their P and dS rows (which the transposed products sum over)
+    // are 0
+    const float row_c =
+        rv ? fmaf(AT_MASK_BIG, a.scale_log2, lse[(long long)(tok0 + r) * a.heads + head]) : INFINITY;
+    const float Di = sDi[r];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int j = g * 8 + k * 2;
-          uint32_t m2 = 0xFFFFFFFFu;
-          float keep0 = 1.0f, keep1 = 1.0f;
-          if (drop) {
-            const uint32_t sg = attn_keep_sum(attn_drop_pair(h0, k), k2);
-            m2 = prmt(sg, 0u, 0xBB99u);
-            keep0 = __uint_as_float(prmt(sg, 0u, 0x9999u) & ks_bits);
-            keep1 = __uint_as_float(prmt(sg, 0u, 0xBBBBu) & ks_bits);
-          }
-          const float p0 = ex2(fmaf(__uint_as_float(r[j]), a.scale_log2, -row_c));
-          const float p1 = ex2(fmaf(__uint_as_float(r[j + 1]), a.scale_log2, -row_c));
-          const float ds0 = p0 * fmaf(__uint_as_float(d[j]), keep0, -Di);
-          const float ds1 = p1 * fmaf(__uint_as_float(d[j + 1]), keep1, -Di);
-          pk[j >> 1] = pack_bf16x2(p0, p1) & m2;
-          dk[j >> 1] = pack_bf16x2(ds0, ds1);
-        }
+    for (int j = 0; j < 16; ++j) {
+      uint32_t m2 = 0xFFFFFFFFu;
+      float keep0 = 1.0f, keep1 = 1.0f;
+      if (drop) {
+        const uint32_t h0 = attn_drop_group(a.drop_key, tok0 + r, a.heads, head, j);
+        const uint32_t sg = attn_keep_sum(attn_drop_pair(h0, fc >> 1), k2);
+        m2 = prmt(sg, 0u, 0xBB99u);
+        keep0 = __uint_as_float(prmt(sg, 0u, 0x9999u) & ks_bits);
+        keep1 = __uint_as_float(prmt(sg, 0u, 0xBBBBu) & ks_bits);
       }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 16; ++j) pk[j] = dk[j] = 0u;
-    }
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      const int u = (c & 1) * 4 + g;
-      const uint32_t in_chunk = i * 128 + ((u ^ (i & 7)) << 4);
-      *reinterpret_cast<uint4*>(sP + (c >> 1) * P_CHUNK + in_chunk) =
-          make_uint4(pk[4 * g], pk[4 * g + 1], pk[4 * g + 2], pk[4 * g + 3]);
-      *reinterpret_cast<uint4*>(sdS + (c >> 1) * (AT_ROWS * 128) + in_chunk) =
-          make_uint4(dk[4 * g], dk[4 * g + 1], dk[4 * g + 2], dk[4 * g + 3]);
+      const int q = 4 * j + 2 * h;
+      const float p0 = ex2(fmaf(s[q], a.scale_log2, -row_c));
+      const float p1 = ex2(fmaf(s[q + 1], a.scale_log2, -row_c));
+      const float ds0 = p0 * fmaf(dp[q], keep0, -Di);
+      const float ds1 = p1 * fmaf(dp[q + 1], keep1, -Di);
+      const uint32_t in_chunk = r * 128 + (((j & 7) ^ (r & 7)) << 4) + fc * 2;
+      *reinterpret_cast<uint32_t*>(sP + (j >> 3) * P_CHUNK + in_chunk) = pack_bf16x2(p0, p1) & m2;
+      *reinterpret_cast<uint32_t*>(sdS + (j >> 3) * (AT_ROWS * 128) + in_chunk) =
+          pack_bf16x2(ds0, ds1);
     }
   }
   fence_proxy_async();
-  tc_fence_before_sync();
   __syncthreads();
 
-  if (threadIdx.x == 0) {
-    tc_fence_after_sync();
+  {
     // dQ[i][d] = sum_j dS[i][j] K[j][d] : A = dS K-major, B = K tile as [k=j][n=d] (MN-major)
-    constexpr uint32_t id_q = make_idesc_bf16(128, 64, 0, 1);
     // dK[j][d] = sum_i dS[i][j] Q[i][d], dV[j][d] = sum_i P[i][j] dO[i][d]:
     //   A = dS^T / P^T = the same smem tiles read MN-major, B = Q / dO tiles MN-major
-    constexpr uint32_t id_t = make_idesc_bf16(128, 64, 1, 1);
+    float dq[32], dk[32], dv[32];
+    wgmma_fence();
 #pragma unroll
     for (int k = 0; k < AT_ROWS / 16; ++k) {
-      const uint64_t ad =
-          make_sw128_desc(smem_u32(sdS) + (k >> 2) * (AT_ROWS * 128) + (k & 3) * 32, 16, 1024);
-      const uint64_t bd = make_sw128_desc(smem_u32(sK) + k * 2048, AT_TILE_BYTES, 1024);
-      umma_f16(tmem, ad, bd, id_q, k > 0 ? 1u : 0u);
+      wgmma_m64n64k16<0, 1>(
+          dq, make_sw128_desc(smem_u32(sdS) + (k >> 2) * (AT_ROWS * 128) + half * 8192 + (k & 3) * 32, 16, 1024),
+          make_sw128_desc(smem_u32(sK) + k * 2048, AT_TILE_BYTES, 1024), k > 0 ? 1u : 0u);
+      wgmma_m64n64k16<1, 1>(
+          dk, make_sw128_desc(smem_u32(sdS) + half * (AT_ROWS * 128) + k * 2048, AT_ROWS * 128, 1024),
+          make_sw128_desc(smem_u32(sQ) + k * 2048, AT_TILE_BYTES, 1024), k > 0 ? 1u : 0u);
+      wgmma_m64n64k16<1, 1>(
+          dv, make_sw128_desc(smem_u32(sP) + half * P_CHUNK + k * 2048, P_CHUNK, 1024),
+          make_sw128_desc(smem_u32(sdO) + k * 2048, AT_TILE_BYTES, 1024), k > 0 ? 1u : 0u);
     }
-#pragma unroll
-    for (int k = 0; k < AT_ROWS / 16; ++k) {
-      const uint64_t ad = make_sw128_desc(smem_u32(sdS) + k * 2048, AT_ROWS * 128, 1024);
-      const uint64_t bd = make_sw128_desc(smem_u32(sQ) + k * 2048, AT_TILE_BYTES, 1024);
-      umma_f16(tmem + 64, ad, bd, id_t, k > 0 ? 1u : 0u);
-    }
-#pragma unroll
-    for (int k = 0; k < AT_ROWS / 16; ++k) {
-      const uint64_t ad = make_sw128_desc(smem_u32(sP) + k * 2048, P_CHUNK, 1024);
-      const uint64_t bd = make_sw128_desc(smem_u32(sdO) + k * 2048, AT_TILE_BYTES, 1024);
-      umma_f16(tmem + 128, ad, bd, id_t, k > 0 ? 1u : 0u);
-    }
-    umma_commit(mma_bar);
-  }
-  mbar_wait(mma_bar, 1);
-  tc_fence_after_sync();
-
-  // rows of dQ (query i), dK / dV (key i) -> dqkv[tok0 + i, {0, H, 2H} + head * 64 ...]: staged in the
-  // (now dead) Q / K / V tiles, then written with coalesced row stores
-#pragma unroll 1
-  for (int part = 0; part < 3; ++part) {
-    uint32_t r0[32];
-    tmem_ld_32x32(t_row + part * 64 + half * 32, r0);
-    tmem_ld_wait();
-    stage_half_row(smem + part * AT_TILE_BYTES, i, half, r0, part == 2 ? keep_scale : a.scale);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(dq);
+    wgmma_fence_acc(dk);
+    wgmma_fence_acc(dv);
+    __syncthreads();     // every operand read has retired: Q / K / V(P) tiles take the results
+    // rows of dQ (query r), dK / dV (key r) -> dqkv[tok0 + r, {0, H, 2H} + head * 64 ...]: staged
+    // in the Q / K / V tiles, then written with coalesced row stores
+    stage_frag64(sQ, wrow0, dq, a.scale, a.scale);
+    stage_frag64(sK, wrow0, dk, a.scale, a.scale);
+    stage_frag64(sV, wrow0, dv, keep_scale, keep_scale);
   }
   // Bias gradient of the QKV projection = column sums of dqkv over the tile's tokens: one more
   // MMA over the staged tiles. A = [dQ | dK] (then [dV | -]) read MN-major (m = feature,
   // k = token), B = 16 identical rows of the token-validity vector (K-major) -> every column of
-  // D holds the column sums, feature m in TMEM lane m: one fp32 atomic per thread replaces the
-  // separate pass over dqkv (hero_colsum_bf16: 76 MB per layer).
+  // D holds the column sums: one fp32 atomic per feature replaces a separate pass over dqkv.
   uint8_t* sB = sdS;
   if (dbias != nullptr) {
-    {
-      const int idx = threadIdx.x;                          // unit (n, chunk, u)
-      const int n = idx >> 4, ch = (idx >> 3) & 1, u = idx & 7;
-      const int k0 = ch * 64 + u * 8;
-      uint32_t w[4];
+    const int idx = threadIdx.x;                          // unit (n, chunk, u)
+    const int n = idx >> 4, ch = (idx >> 3) & 1, u = idx & 7;
+    const int k0 = ch * 64 + u * 8;
+    uint32_t w[4];
 #pragma unroll
-      for (int e = 0; e < 4; ++e)
-        w[e] = ((k0 + 2 * e < ntok) ? 0x3F80u : 0u) | ((k0 + 2 * e + 1 < ntok) ? 0x3F800000u : 0u);
-      *reinterpret_cast<uint4*>(sB + ch * 2048 + n * 128 + ((u ^ (n & 7)) << 4)) =
-          make_uint4(w[0], w[1], w[2], w[3]);
-    }
-    fence_proxy_async();
+    for (int e = 0; e < 4; ++e)
+      w[e] = ((k0 + 2 * e < ntok) ? 0x3F80u : 0u) | ((k0 + 2 * e + 1 < ntok) ? 0x3F800000u : 0u);
+    *reinterpret_cast<uint4*>(sB + ch * 2048 + n * 128 + ((u ^ (n & 7)) << 4)) =
+        make_uint4(w[0], w[1], w[2], w[3]);
   }
-  tc_fence_before_sync();
+  fence_proxy_async();
   __syncthreads();
-  if (dbias != nullptr && threadIdx.x == 0) {
-    tc_fence_after_sync();
-    constexpr uint32_t id_c = make_idesc_bf16(128, 16, 1, 0);
-#pragma unroll
-    for (int grp = 0; grp < 2; ++grp) {
-#pragma unroll
-      for (int k = 0; k < AT_ROWS / 16; ++k) {
-        const uint64_t ad = make_sw128_desc(smem_u32(smem) + grp * 2 * AT_TILE_BYTES + k * 2048,
-                                            AT_TILE_BYTES, 1024);
-        const uint64_t bd = make_sw128_desc(smem_u32(sB) + (k >> 2) * 2048 + (k & 3) * 32, 16, 1024);
-        umma_f16(tmem + 192 + grp * 16, ad, bd, id_c, k > 0 ? 1u : 0u);
-      }
-    }
-    umma_commit(mma_bar);
-  }
   store_tiles(smem, 3, dqkv + (long long)tok0 * (3 * a.H) + head * AT_D, 3LL * a.H, a.H, ntok);
   if (dbias != nullptr) {
-    mbar_wait(mma_bar, 0);       // third phase of this barrier
-    tc_fence_after_sync();
-    const float cs = __uint_as_float(tmem_ld_32x1(t_row + 192 + half * 16));
-    tmem_ld_wait();
     float* db = dbias + head * AT_D;
-    if (half == 0) {
-      if (i < AT_D) atomicAdd(db + i, cs);                 // dQ feature i
-      else atomicAdd(db + a.H + (i - AT_D), cs);           // dK feature i - 64
-    } else if (i < AT_D) {
-      atomicAdd(db + 2 * a.H + i, cs);                     // dV feature i
+    // warpgroup g: features [64g, 64g + 64) of [dQ | dK] (tiles 0, 1), then warpgroup 0 alone: dV
+#pragma unroll 1
+    for (int grp = 0; grp < 2 - half; ++grp) {
+      float cs[8];
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < AT_ROWS / 16; ++k)
+        wgmma_m64n16k16<1, 0>(
+            cs, make_sw128_desc(smem_u32(smem) + (grp * 2 + half) * AT_TILE_BYTES + k * 2048, AT_TILE_BYTES, 1024),
+            make_sw128_desc(smem_u32(sB) + (k >> 2) * 2048 + (k & 3) * 32, 16, 1024), k > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_acc(cs);
+      if ((lane & 3) == 0) {
+        const int f = (warp & 3) * 16 + (lane >> 2);       // feature of d[0]; d[2]: f + 8
+        float* dst = db + (grp == 1 ? 2 * a.H : (half ? a.H : 0));
+        atomicAdd(dst + f, cs[0]);
+        atomicAdd(dst + f + 8, cs[2]);
+      }
     }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem, 256);
   }
 }
 
@@ -923,7 +781,7 @@ extern "C" int hero_attn_fwd(const void* qkv, const int32_t* tile_tok0, const in
     return rc;
   CUtensorMap tm;
   if (int rc = encode_tmap_2d_bf16(&tm, qkv, 3LL * a.H, n_tok, 3LL * a.H, AT_D, AT_ROWS)) return rc;
-  const int smem = 3 * AT_TILE_BYTES + AT_MASK_BYTES + 64;
+  const int smem = 3 * AT_TILE_BYTES + AT_P_BYTES + AT_MASK_BYTES + 64;
   static bool configured = false;
   if (!configured) {
     HERO_CUDA_CHECK(cudaFuncSetAttribute(attn_tc_fwd_kernel,
@@ -972,7 +830,7 @@ extern "C" int hero_attn_bwd(const void* qkv, const int32_t* tile_tok0, const in
   if (int rc = encode_tmap_2d_bf16(&tq, qkv, 3LL * a.H, n_tok, 3LL * a.H, AT_D, AT_ROWS)) return rc;
   if (int rc = encode_tmap_2d_bf16(&td, dctx, a.H, n_tok, a.H, AT_D, AT_ROWS)) return rc;
   if (int rc = encode_tmap_2d_bf16(&to, ctx, a.H, n_tok, a.H, AT_D, AT_ROWS)) return rc;
-  const int smem = 5 * AT_TILE_BYTES + AT_P_BYTES + 64;
+  const int smem = 5 * AT_TILE_BYTES + AT_P_BYTES + 64 + AT_ROWS * 4;
   static bool configured = false;
   if (!configured) {
     HERO_CUDA_CHECK(cudaFuncSetAttribute(attn_tc_bwd_kernel,

@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld), fences. No CUTLASS dependency.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma, fences.
+// No CUTLASS dependency.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -94,177 +94,92 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, ui
       : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers bf16 inputs with fp32 accumulate.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued MMAs of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (lane = row).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// one fp32 column: thread (lane) <- its own row
-__device__ __forceinline__ uint32_t tmem_ld_32x1(uint32_t taddr) {
-  uint32_t r;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(r) : "r"(taddr) : "memory");
-  return r;
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// ---------------------------------------------------------------- CTA pairs (cta_group::2)
-// Two CTAs of a cluster (ranks 0/1 on one TPC) run ONE 256-row MMA: each holds half of A (its 128
-// rows) and half of B (128 of the 256 columns) in its own smem, the leader (rank 0) issues the
-// instruction, each CTA's TMEM receives its 128 accumulator rows. Halves the smem operand traffic
-// per MAC, which is what bounds the single-CTA kernel.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// In a CTA pair the shared::cluster address of the leader's copy of a smem object is the local
-// shared::cta address with bit 24 cleared (CUTLASS Sm100MmaPeerBitMask).
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-// Relaxed: the only thing this arrival publishes is "my tcgen05.ld's of the accumulator have
-// completed", which the preceding tcgen05.wait::ld + tcgen05.fence::before_thread_sync already
-// order. The default .release at cluster scope compiles to MEMBAR.ALL.CTA + ERRBAR, which waits
-// for every outstanding global store / fp32 atomic of the epilogue (13 % of the samples of a
-// pair-mode GEMM in profiles/r01d).
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(
-                   smem_u32(bar) & kPeerBitMask)
-               : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const void* tmap, uint64_t* bar,
-                                                int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_2sm(void* smem_dst, const void* tmap, uint64_t* bar,
-                                                int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1),
-      "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive (once the issued MMAs retire) on the barrier at the same smem offset in BOTH CTAs.
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 "
-      "[%0], %1;" ::"r"(smem_u32(bar)),
-      "h"(static_cast<uint16_t>(3))
-      : "memory");
-}
-
-// Shared-memory matrix descriptor (sm_100 "version 1"), 128-byte swizzle.
+// ---------------------------------------------------------------- wgmma (sm_90a)
+// Shared-memory matrix descriptor for wgmma, 128-byte swizzle:
 //   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version = 1
-//   bits [61,64) layout type (2 = SWIZZLE_128B)
+//   bits [32,46) stride byte offset >> 4   bits [62,64) layout type (1 = SWIZZLE_128B)
+// K-major operands: 8-row groups SBO = 1024 B apart, LBO unused (encoded 1).
+// MN-major operands: 64-element MN atoms LBO bytes apart, 8-k groups SBO = 1024 B apart.
 __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr, uint32_t lbo_bytes,
                                                     uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
-// Instruction descriptor for kind::f16, bf16 x bf16 -> fp32.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major,
-                                                       int b_mn_major) {
-  return (1u << 4)                                   // D format: f32
-         | (1u << 7)                                 // A format: bf16
-         | (1u << 10)                                // B format: bf16
-         | (static_cast<uint32_t>(a_mn_major) << 15) // A major (0 = K, 1 = MN)
-         | (static_cast<uint32_t>(b_mn_major) << 16) // B major
-         | (static_cast<uint32_t>(N >> 3) << 17)     // N / 8
-         | (static_cast<uint32_t>(M >> 4) << 24);    // M / 16
+// Warpgroup-collective: every thread of the 128-thread warpgroup executes these.
+__device__ __forceinline__ void wgmma_fence() {
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+}
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+}
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// Keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs.
+template <int R>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 inputs, fp32 accumulators in registers.
+// TA / TB: 0 = K-major, 1 = MN-major operand. Accumulator fragment of thread t of the warpgroup
+// (warp w = t / 32, lane l): d[4j + 2h + e] = D[16w + l / 4 + 8h][8j + 2(l % 4) + e].
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t adesc, uint64_t bdesc,
+                                                uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+      "%8, %9, p, 1, 1, %11, %12;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t adesc, uint64_t bdesc,
+                                                uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, %35, %36;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc,
+                                                uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, %67, %68;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
 }
 
 // ---------------------------------------------------------------- programmatic dependent launch
 // Kernels launched with the programmatic-stream-serialization attribute may start while the
 // previous kernel in the stream is still draining: everything before pdl_wait() (barrier init,
-// TMEM allocation, descriptor prefetch) overlaps that tail; pdl_wait() blocks until the previous
+// descriptor prefetch) overlaps that tail; pdl_wait() blocks until the previous
 // grid has completed and its writes are visible. pdl_launch_dependents() lets the NEXT kernel
 // begin its own prologue early.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -364,7 +279,7 @@ __device__ __forceinline__ bool attn_drop_keep(uint32_t key, uint32_t threshold,
   return lane >= (threshold >> 17);
 }
 
-// exp2 on the MUFU unit (one op per element is the epilogue's throughput budget on sm_100).
+// exp2 on the MUFU unit (one op per element).
 __device__ __forceinline__ float fast_ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -403,61 +318,6 @@ __device__ __forceinline__ float gelu_erf_with_grad(float x, float& dgelu) {
   dgelu = fmaf(x, pdf, cdf);
   return fmaxf(x, 0.f) - fabsf(x * e);
 }
-// ---- packed fp32x2 arithmetic (sm_100 FFMA2 / FMUL2 / FADD2: one issue slot, two lanes) ----
-__device__ __forceinline__ uint64_t f2_pack(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void f2_unpack(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t f2_mul(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ uint64_t f2_add(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ uint64_t f2_splat(float v) { return f2_pack(v, v); }
-
-// gelu_erf_with_grad on two values at once: the polynomial, the pdf exponent and the final
-// combinations run as packed FFMA2 (25 issue slots per pair instead of 38).
-__device__ __forceinline__ void gelu_erf_with_grad2(float& x0, float& x1, float& d0, float& d1) {
-  const float a0 = fminf(fabsf(x0), 8.4852814f), a1 = fminf(fabsf(x1), 8.4852814f);
-  const uint64_t ax = f2_pack(a0, a1);
-  uint64_t p = f2_splat(3.1522031349595636e-05f);
-  p = f2_fma(p, ax, f2_splat(-0.000753118481952697f));
-  p = f2_fma(p, ax, f2_splat(0.00801779329776764f));
-  p = f2_fma(p, ax, f2_splat(-0.05329384654760361f));
-  p = f2_fma(p, ax, f2_splat(-0.4588814675807953f));
-  p = f2_fma(p, ax, f2_splat(-1.1511543989181519f));
-  p = f2_fma(p, ax, f2_splat(-1.0f));
-  float p0, p1;
-  f2_unpack(p, p0, p1);
-  const float e0 = fast_ex2(p0), e1 = fast_ex2(p1);
-  const uint64_t x = f2_pack(x0, x1);
-  const uint64_t t = f2_fma(f2_mul(x, x), f2_splat(-0.72134752044448170f),
-                            f2_splat(-1.3257480647361592f));
-  float t0, t1;
-  f2_unpack(t, t0, t1);
-  const uint64_t pdf = f2_pack(fast_ex2(t0), fast_ex2(t1));
-  const uint64_t cdf = f2_pack(0.5f + copysignf(0.5f - e0, x0), 0.5f + copysignf(0.5f - e1, x1));
-  f2_unpack(f2_fma(x, pdf, cdf), d0, d1);
-  float xe0, xe1;
-  f2_unpack(f2_mul(x, f2_pack(e0, e1)), xe0, xe1);
-  x0 = fmaxf(x0, 0.f) - fabsf(xe0);
-  x1 = fmaxf(x1, 0.f) - fabsf(xe1);
-}
-
 __device__ __forceinline__ float gelu_erf_grad(float x) {
   float d;
   (void)gelu_erf_with_grad(x, d);

@@ -432,7 +432,7 @@ __device__ __forceinline__ float block_sum_256(float v, float* red) {
 
 // (gamma / beta are re-read per row - 35 KB that stay in L1 - instead of living in 48 registers:
 // at 64 registers four CTAs fit per SM, and one row per CTA in flight needs that many to cover
-// the HBM latency: 36 -> see profiles/r02_ln_bench.txt)
+// the HBM latency)
 __global__ void __launch_bounds__(LNW_THREADS, 4)
 ln_fwd_wide_kernel(const hero_ln_args a) {
   pdl_wait();

@@ -1,7 +1,7 @@
 // Native layer runtime: launches the whole per-layer kernel sequence of a BertLayer stack
 // (forward and backward) from C++, so the host cost per step is a handful of calls instead of
 // hundreds of Python->ctypes round trips. Pure orchestration: every arithmetic step is one of the
-// kernels behind the C-ABI (gemm_tcgen05, attention_tc, rowwise).
+// kernels behind the C-ABI (gemm_wgmma, attention_tc, rowwise).
 #include <stdlib.h>
 #include <string.h>
 

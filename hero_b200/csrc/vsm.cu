@@ -3,7 +3,7 @@
 // the reference), fused so the head is a handful of launches with no host round trip:
 //
 //   video-level scores   q^ = q / max(|q|, eps), c^ = c / max(|c|, eps)        (l2norm_split)
-//                        S[m, (n, l)] = q^_m . c^_{n,l}                          (tcgen05 GEMM, split-bf16)
+//                        S[m, (n, l)] = q^_m . c^_{n,l}                          (wgmma GEMM, split-bf16)
 //                        score[m, n] = max_l mask_logits(S[m, n, l], mask[n, l]) (masked_max)
 //   span logits          sim[b, l] = query_b . ctx_{b,l};  st / ed = conv1d_k(sim) masked
 //

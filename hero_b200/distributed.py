@@ -1,5 +1,5 @@
 """Data-parallel plumbing: the function names of the reference's utils/distributed.py on top of
-torch.distributed (NCCL over NVLink 5 / NVSwitch on the B200 box, gloo in CPU tests) instead of
+torch.distributed (NCCL over NVLink / NVSwitch on a multi-GPU node, gloo in CPU tests) instead of
 Horovod.
 
 Semantics kept from the reference (SURVEY.md Appendix D.8):
@@ -590,13 +590,9 @@ def overlapped_exchange(flat, transport="none", **kw):
     GradBucketer ("p2p": buckets travel as peer copies during backward, "nccl": through a capped
     communicator).
 
-    B200 / NVSwitch, 430 MB of fp32 gradients, 6.4-6.5 ms of compute per step, ms per step:
-      N = 2: bucketer 7.23-7.34 device-resident but 7.96 end to end (its ~100 extra host-side
-             enqueues per step double the host time of a step), all-reduce after backward 7.32;
-      N = 4: bucketer 8.23, all-reduce after backward 7.65 - every bucket costs 2 (N-1) copies and
-             signals per rank, and NCCL's all-reduce grows by only 0.3 ms from N = 2 to N = 4.
-    The bucketer hides its exchanges completely (HERO_DP_TIMING=1) but the 41 % of the bytes that
-    become final only when backward ends stay exposed either way, so it is opt-in."""
+    The bucketer pays ~100 extra host-side enqueues per step and 2 (N-1) copies and signals per
+    bucket per rank, and the 41 % of the bytes that become final only when backward ends stay
+    exposed either way, so it is opt-in (not measured on H100)."""
     if size() <= 1 or transport in (None, "none"):
         return None
     return GradBucketer(flat, transport=transport, **kw)

@@ -489,7 +489,7 @@ def gather_rows(src, idx, inv_idx):
 # ---------------------------------------------------------------------------------------------
 class _VsmVideoScores(torch.autograd.Function):
     """(Nq, Nv) = max over a clip's valid frames of the cosine of every query with every frame
-    (model/pretrain.py:364-413 after the cross-rank gather): l2norm (split-bf16) -> tcgen05 GEMM
+    (model/pretrain.py:364-413 after the cross-rank gather): l2norm (split-bf16) -> wgmma GEMM
     q^ . c^ with split-bf16 operands -> masked max; backward through the arg-max frames."""
 
     @staticmethod
@@ -568,7 +568,7 @@ def vsm_span_logits(query, frames, mask, w_st, w_ed):
 # ---------------------------------------------------------------------------------------------
 class _LmHeadCrossEntropy(torch.autograd.Function):
     """loss[r] = cross_entropy(h[r] @ E^T + bias, label[r]) over the first n_valid vocabulary
-    entries (model/layers.py:347-354 decoder + model/encoder.py:366-372), as ONE tcgen05 GEMM whose
+    entries (model/layers.py:347-354 decoder + model/encoder.py:366-372), as ONE wgmma GEMM whose
     epilogue keeps only online-softmax partials; the backward recomputes the logits tile by tile
     and emits d logits in bf16, which feeds the tied-embedding weight gradient (fp32 accumulate
     into the embedding table's gradient), the bias gradient and d h.

@@ -2,7 +2,7 @@
 
 `PrefetchLoader` keeps the reference's interface (data/loader.py:89-144: wrap a loader, iterate
 device batches, transfers overlap compute on a side stream) with two changes that matter at
-B200 step times (8 ms per 32-clip step, 112 MB of frame features per step):
+step times of a few milliseconds per 32-clip step with 112 MB of frame features per step:
 
 * batches land in a small ring of preallocated device buffers (`BatchStager`) instead of fresh
   `.cuda()` allocations guarded by `record_stream`: cross-stream frees keep the caching allocator

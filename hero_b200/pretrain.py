@@ -11,7 +11,7 @@ classes, so `train_vcmr.py` / `pretrain.py` and their checkpoints keep working. 
   (`distributed.vsm_allgather`, same forward/backward contract as the Horovod-based
   `VsmAllgather`, model/pretrain.py:427-451);
 * the head's device work after the query pooling is fused (hero_b200/csrc/vsm.cu): the
-  video-level scores are l2norm -> split-bf16 tcgen05 GEMM -> masked max (3 launches forward, 2
+  video-level scores are l2norm -> split-bf16 wgmma GEMM -> masked max (3 launches forward, 2
   backward, instead of ~15 + ~25 torch kernels), the span logits one kernel each way; nothing in
   the training-mode forward reads a value back to the host (clips are padded to `max_clip_len`
   for the cross-rank gather instead of exchanging lengths; equal per-rank query / clip counts are

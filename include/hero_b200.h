@@ -1,5 +1,5 @@
 /*
- * hero_b200 C-ABI — the drop-in boundary of the B200-native HERO encoder hot path.
+ * hero_b200 C-ABI — the drop-in boundary of the H100-native (sm_90a) HERO encoder hot path.
  *
  * The reference (linjieli222/HERO) has no FFI layer: its boundary is the Python nn.Module
  * surface of model/{layers,embed,encoder,model}.py. Each entry point below replaces the device
@@ -37,7 +37,7 @@ typedef enum hero_status {
 /* Library / device info. */
 const char* hero_last_error(void);
 int hero_version(void);
-/* Returns SM count of the current device (148 on B200) or a negative hero_status. */
+/* Returns SM count of the current device (132 on H100 SXM) or a negative hero_status. */
 int hero_sm_count(void);
 /* Size every persistent kernel for at most n SMs (0 = all). The GEMMs run one CTA per SM; while a
  * communication kernel (NCCL) holds some SMs a full-size grid would need a second wave for the
@@ -46,7 +46,7 @@ int hero_sm_count(void);
 int hero_set_sm_limit(int32_t n);
 
 /* ------------------------------------------------------------------------------------------
- * GEMM family (tcgen05 / TMEM / TMA).   D[M,N] = epilogue( A · B^T-like contraction )
+ * GEMM family (wgmma / TMA).   D[M,N] = epilogue( A · B^T-like contraction )
  *
  * Replaces every nn.Linear on the path — model/layers.py:125-127 (Q,K,V), :176 (attn out),
  * :237 (FFN up + gelu :16-25), :251 (FFN down), model/embed.py:112 (img_linear),
@@ -98,10 +98,10 @@ typedef struct hero_gemm_args {
   uint32_t drop_threshold; /* 0 = no dropout; else p * 2^32 */
   uint32_t drop_key;
   float drop_scale;        /* 1 / (1 - p) */
-  int32_t block_n;         /* 0 = auto, else 128 or 256 */
+  int32_t block_n;         /* 0 = auto, 128 or 256; sm_90 runs every GEMM on 128 x 128 tiles */
   int32_t k_splits;        /* 0 = auto (only > 1 when out_f32_accumulate) */
-  int32_t cta_pair;        /* 0 = auto, 1 = single-CTA tiles, 2 = force CTA pairs (cta_group::2,
-                              256 x 256 tiles; needs block_n 256) */
+  int32_t cta_pair;        /* 0 = auto, 1 = single-CTA tiles, 2 = CTA pairs; sm_90 has no
+                              paired-CTA MMA, so every value runs single-CTA tiles */
   int32_t resid_f32;       /* resid is f32 [m, ld_resid] (needs out_f32_store) */
   int32_t out_f32_store;   /* out is f32 [m, ld_out], plain store (act 0 only; ld_out % 4 == 0) */
   /* Split-bf16 operands (both or neither; same layout / leading dims as a, b): the contraction
@@ -224,7 +224,7 @@ int hero_ln_fwd(const hero_ln_args* args, void* stream);
 int hero_ln_bwd(const hero_ln_args* args, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * Variable-length multi-head self-attention over packed sequences (tcgen05 / TMEM / TMA).
+ * Variable-length multi-head self-attention over packed sequences (wgmma / TMA).
  *
  * Replaces model/layers.py:129-160 (transpose_for_scores, QK^T/sqrt(d) + additive -10000 key
  * mask, softmax, dropout on probabilities, P·V, head merge) and its backward. Only valid tokens
@@ -241,7 +241,7 @@ int hero_ln_bwd(const hero_ln_args* args, void* stream);
  *                                           straddles two tiles
  *   seq_lo[n_tok], seq_hi[n_tok]            [lo, hi) packed-token range of each token's sequence
  * One CTA per (tile, head): S = QK^T and O = PV (forward), S, dP, dQ, dK, dV (backward) are
- * tcgen05.mma contractions with fp32 accumulators in TMEM; probabilities never reach HBM.
+ * wgmma contractions with fp32 accumulators in registers; probabilities never reach HBM.
  * The "own sequence only" mask is itself a tensor-core product: one extra K = 16 step adds 16384
  * to every same-sequence (query, key) score (membership matrix x its transpose), which leaves the
  * row's softmax unchanged and sends every other column's exp2 to exactly 0 - no per-element

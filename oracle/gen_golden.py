@@ -1,13 +1,13 @@
 """Generates tests/golden/*.npz by running the UNMODIFIED reference modules on CPU.
 
-Runs only in the build container (needs /root/reference, which does not exist on the GPU box).
+Needs a checkout of the reference, given as HERO_REFERENCE=<path>; the GPU tests never run it.
 The reference is imported, never copied: apex / horovod / lmdb ... are replaced by in-memory
 stubs (SURVEY.md Appendix B), `FusedLayerNorm` by `torch.nn.LayerNorm` (same semantics and
 parameter names). Fixtures hold outputs (and, for tiny configs, the weights and inputs); the
 full-dimension fixtures regenerate weights/inputs from seeds via `oracle.hero_oracle.seeded_weights`
 and `hero_b200.synth`, so the files stay small.
 
-    python oracle/gen_golden.py
+    HERO_REFERENCE=<checkout of linjieli222/HERO> python oracle/gen_golden.py
 """
 import itertools
 import json
@@ -20,7 +20,7 @@ import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.environ.get("HERO_REFERENCE", "/root/reference")
+REF = os.environ.get("HERO_REFERENCE", "")
 sys.path.insert(0, ROOT)
 
 from hero_b200 import synth  # noqa: E402
@@ -49,6 +49,8 @@ def install_stubs():
     mod("toolz.sandbox", unzip=lambda seq: zip(*seq))
     mod("cytoolz", concat=itertools.chain.from_iterable)
     mod("tensorboardX", SummaryWriter=object)
+    if not os.path.isfile(os.path.join(REF, "model", "model.py")):
+        raise SystemExit("set HERO_REFERENCE to a checkout of linjieli222/HERO")
     sys.path.insert(0, REF)
 
 

@@ -1,5 +1,5 @@
 """Pins the CPU oracle against outputs of the unmodified reference (tests/golden/*.npz, produced
-by oracle/gen_golden.py in the build container). fp32 on both sides -> tight tolerance."""
+by oracle/gen_golden.py from the reference). fp32 on both sides -> tight tolerance."""
 import numpy as np
 import torch
 

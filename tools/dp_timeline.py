@@ -46,7 +46,7 @@ if rank == 0:
     print(f"step span {(t1 - t0) / 1e3:.3f} ms, {len(evs)} device activities")
     comp_end = max(e.time_range.end for e in evs if "nccl" not in e.name.lower())
     print(f"last compute kernel ends at {(comp_end - t0) / 1e3:.3f} ms")
-    bwd_end = max(e.time_range.end for e in evs if "hero::" in e.name or "gemm_tcgen05" in e.name)
+    bwd_end = max(e.time_range.end for e in evs if "hero::" in e.name or "gemm_wgmma" in e.name)
     print(f"last hero kernel ends at {(bwd_end - t0) / 1e3:.3f} ms; activities after "
           f"{(bwd_end - t0) / 1e3 - 0.3:.3f} ms:")
     for e in sorted(evs, key=lambda e: e.time_range.start):

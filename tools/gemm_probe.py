@@ -1,4 +1,4 @@
-"""Times the tcgen05 GEMM on the encoder's shapes (CUDA events, L2 flushed between reps)."""
+"""Times the wgmma GEMM on the encoder's shapes (CUDA events, L2 flushed between reps)."""
 import sys, os, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,6 +1,6 @@
 """Aggregate an `ncu --metrics gpu__time_duration.sum --csv` launch list by kernel.
 
-    python tools/launch_summary.py profiles/r01_launches_bench_step.csv [--step]
+    python tools/launch_summary.py launches.csv [--step]
 
 --step: keep exactly one training step = the launches from one zeroing of the flat gradient
 buffer (the only > 30 us FillFunctor<float> of a step) up to the next one.

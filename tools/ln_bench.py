@@ -25,7 +25,7 @@ def timeit(fn, n=40):
 
 
 for M in (16512, 3200):
-    R = 12 if M > 10000 else 40           # rotate through R buffer sets (> 126 MB of L2)
+    R = 12 if M > 10000 else 40           # rotate through R buffer sets (> 50 MB of L2)
     xs = [torch.randn(M, H, device=dev).bfloat16() for _ in range(R)]
     dys = [torch.randn(M, H, device=dev).bfloat16() for _ in range(R)]
     ys = [torch.empty(M, H, dtype=torch.bfloat16, device=dev) for _ in range(R)]

@@ -1,4 +1,4 @@
-"""Encoder-shaped GEMM launches for `ncu --set full --import-source on` (see profiles/README.md):
+"""Encoder-shaped GEMM launches for `ncu --set full --import-source on`:
 the five epilogue families at the cross-modal (M = 16512) and temporal (M = 3200) token counts."""
 import os
 import sys

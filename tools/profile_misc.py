@@ -1,4 +1,4 @@
-"""Attention / LayerNorm launches at bench shapes for `ncu --set full` (see profiles/README.md)."""
+"""Attention / LayerNorm launches at bench shapes for `ncu --set full`."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
