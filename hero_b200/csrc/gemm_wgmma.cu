@@ -1,21 +1,26 @@
 // Persistent warp-specialised bf16 GEMM for sm_90a: TMA -> 128B-swizzled smem ring ->
 // wgmma (fp32 accumulators in registers) -> fused epilogue.
 //
-// One CTA per SM, 9 warps, 128 x 128 tiles:
-//   warps 0..7  two consumer warpgroups; warpgroup g owns rows [64g, 64g + 64) of the 128-row tile.
-//               Main loop: wgmma.m64nNk16 straight from the smem ring, one MMA group in flight
-//               (the stage it read is released when the next group has been issued).
-//               Epilogue, per warp (16 rows) and per slab (16 rows x 64 bf16 columns, or 16 rows x
-//               32 fp32 columns when the residual stream is involved — always 16 x 128 B = one 2 KB
-//               swizzled smem slab), on the accumulator fragment itself:
-//                 bias -> activation -> dropout -> residual -> pack -> smem -> TMA store
-//               Everything that comes from or goes to HBM in tiles moves by TMA: the residual /
-//               saved-derivative slab is prefetched one slab ahead into a warp-private smem slab
-//               (its own mbarrier), outputs leave through double-buffered slabs so a store never
-//               waits for the previous one to drain. No CTA-wide barrier in the epilogue.
-//   warp 8      TMA producer (one lane).
-// Pipeline: smem full/empty ring (TMA <-> MMA); the producer runs ahead into the next tile while
-// the consumers run the epilogue of the current one.
+// One CTA per SM, three warpgroups (384 threads), 128 x 128 tiles, ping-pong consumers:
+//   WG0        TMA producer (one lane); the warpgroup gives its registers away (setmaxnreg 40).
+//   WG1, WG2   consumers (setmaxnreg 232). Consumer WG w takes the CTA's local tiles j with
+//              j = w (mod 2), each a whole 128 x 128 tile (128 fp32 accumulators per thread).
+//              Main loop: per k16 step two wgmma.m64n128k16 (rows 0-63, rows 64-127) straight
+//              from the smem ring, one MMA group in flight (the stage it read is released when
+//              the next group has been issued). The two WGs take the tensor cores in turn: a
+//              WG starts its main loop once the other has issued the previous tile's last MMAs
+//              (a pair of named barriers), so one WG's epilogue runs under the other's MMAs.
+//              Epilogue, per warp (16 rows in each 64-row half of the tile) and per slab (16 rows
+//              x 64 bf16 columns, or 16 rows x 32 fp32 columns when the residual stream is
+//              involved — always 16 x 128 B = one 2 KB swizzled smem slab), on the accumulator
+//              fragment itself:
+//                bias -> activation -> dropout -> residual -> pack -> smem -> TMA store
+//              Everything that comes from or goes to HBM in tiles moves by TMA: the residual /
+//              saved-derivative slab is prefetched one slab ahead into a warp-private smem slab
+//              (its own mbarrier), outputs leave through double-buffered slabs so a store never
+//              waits for the previous one to drain. No CTA-wide barrier in the epilogue.
+// Pipeline: smem full/empty ring (TMA <-> MMA); each stage is consumed by the one WG that owns
+// its tile. The producer runs ahead into the next tile while a consumer runs its epilogue.
 //
 // Replaces the cuBLAS calls behind nn.Linear in model/layers.py:125-127,176,237,251,
 // model/embed.py:112 and model/layers.py:82-90 (reference), forward and backward.
@@ -33,13 +38,15 @@
 namespace hero {
 
 constexpr int BLOCK_M = 128;
-// 128 accumulator columns per consumer thread-row fit the register file beside the fused epilogue
-// without spills; 256 (64 more fp32 registers per thread) does not at 9 warps per CTA.
+// A consumer thread holds the whole 128 x 128 tile's fragment (128 fp32 accumulators) beside the
+// fused epilogue's working set within its 232 registers.
 constexpr int BLOCK_N = 128;
 constexpr int BLOCK_K = 64;   // 64 bf16 = 128 bytes = one swizzle span
 constexpr int WG_K = 16;      // K of one wgmma
-constexpr int NUM_EPI_WARPS = 8;                       // = the consumer warps
-constexpr int NUM_THREADS = NUM_EPI_WARPS * 32 + 32;   // + the TMA producer warp
+constexpr int NUM_EPI_WARPS = 8;                       // = the consumer warps (WG1, WG2)
+constexpr int NUM_THREADS = 3 * 128;                   // producer WG + two consumer WGs
+constexpr int PRODUCER_REGS = 40;                      // 40 * 128 + 232 * 256 <= 64 K registers
+constexpr int CONSUMER_REGS = 232;
 constexpr int SLAB_ROWS = 16;                          // rows of a warp's accumulator fragment
 constexpr int SLAB_BYTES = SLAB_ROWS * 128;            // 16 rows x 128 B, swizzle-128B
 constexpr int SMEM_LIMIT = 232448;                     // 227 KB opt-in dynamic shared memory per CTA
@@ -142,6 +149,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
   static_assert(ACT != ACT_GELU_GRAD || RES == RES_BF16, "GELU' multiplier arrives as a bf16 slab");
   static_assert(OUT != OUT_F32_ATOMIC || RES == RES_NONE, "split-K accumulation takes no residual");
   static_assert((ACT == ACT_CE) == (OUT == OUT_NONE), "the CE forward epilogue stores no tile");
+  static_assert(RES == RES_NONE || OUT == OUT_BF16 || OUT == OUT_F32,
+                "the residual slab is refilled after the staged store of the previous slab");
 
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0u) __trap();  // swizzle-128B atoms need a 1024 B aligned base
@@ -153,14 +162,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == NUM_EPI_WARPS && lane == 0) {
+  if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
     if (OUT != OUT_F32_ATOMIC && OUT != OUT_NONE) tma_prefetch_desc(&tmap_out);
     if (RES) tma_prefetch_desc(&tmap_res);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], NUM_EPI_WARPS);   // one arrive per consumer warp
+      mbar_init(&empty_bar[i], 4);   // one arrive per warp of the consumer WG that owns the tile
     }
     for (int i = 0; i < NUM_EPI_WARPS; ++i) mbar_init(&res_bar[i], 1);
     fence_barrier_init();
@@ -175,17 +184,18 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
   const int first_tile = (int)blockIdx.x;
   const int tile_step = (int)gridDim.x;
 
-  if (warp == NUM_EPI_WARPS) {
+  if (warp < 4) {
     // ------------------------------------------------------------- TMA producer
-    if (lane == 0) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == 0 && lane == 0) {
       uint32_t it = 0;
       for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
         const int ks = tile % s.k_splits;
         const int t2 = tile / s.k_splits;
         const int n_blk = t2 % s.num_n_blocks;
         const int m_blk = t2 / s.num_n_blocks;
-        const int kb0 = (int)(((long long)ks * s.k_blocks) / s.k_splits);
-        const int kb1 = (int)(((long long)(ks + 1) * s.k_blocks) / s.k_splits);
+        const int kb0 = ks * s.k_blocks / s.k_splits;
+        const int kb1 = (ks + 1) * s.k_blocks / s.k_splits;
         for (int pass = 0; pass < s.k_passes; ++pass) {
           // split-bf16 passes: (A_hi, B_hi), (A_lo, B_hi), (A_hi, B_lo)
           const CUtensorMap* ma = (pass == 1) ? &tmap_a_lo : &tmap_a;
@@ -211,352 +221,388 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
     }
   } else {
     // ------------------------------------------------------------- consumer warpgroups
-    const int wg = warp >> 2;
-    const int row_off = wg * 64 + (warp & 3) * SLAB_ROWS;   // this warp's 16 rows of the tile
+    setmaxnreg_inc<CONSUMER_REGS>();
+    const int cw = warp - 4;            // consumer warp 0..7: staging slabs, residual mbarrier
+    const int wg = cw >> 2;             // 0 = WG1, 1 = WG2
+    const int row_off = (cw & 3) * SLAB_ROWS;   // this warp's 16 rows in each 64-row half
     const int fr = lane >> 2;          // fragment rows fr, fr + 8 of the warp's 16
     const int fc = (lane & 3) * 2;     // fragment columns 8j + fc, 8j + fc + 1
-    uint8_t* stage0 = smem + Cfg::STAGING_OFFSET + warp * Cfg::SLABS_PER_WARP * SLAB_BYTES;
+    uint8_t* stage0 = smem + Cfg::STAGING_OFFSET + cw * Cfg::SLABS_PER_WARP * SLAB_BYTES;
     uint8_t* out_slab = stage0;                                            // N_OUT_BUF slabs
     uint8_t* aux_slab = stage0 + Cfg::N_OUT_BUF * SLAB_BYTES;             // AUX slab
     uint8_t* res_slab = stage0 + (Cfg::N_OUT_BUF + Cfg::AUX) * SLAB_BYTES;
-    uint64_t* my_res_bar = &res_bar[warp];
+    uint64_t* my_res_bar = &res_bar[cw];
     const bool has_aux = Cfg::AUX && e.has_aux;
     const bool has_bias = (e.bias != nullptr);
     // K-major: 8-row groups 1024 B apart (SBO), LBO unused (encoded 1).
     // MN-major: 64-element MN chunks BLOCK_K*128 B apart (LBO), 8-k groups 1024 B apart (SBO).
-    // Warpgroup g's 64 rows of A start 8 KB into the stage in both layouts.
+    // Rows 64..127 of A start 8 KB into the stage in both layouts.
     constexpr uint32_t A_LBO = A_MN ? BLOCK_K * 128 : 16;
     constexpr uint32_t B_LBO = B_MN ? BLOCK_K * 128 : 16;
     constexpr uint32_t A_KSTEP = A_MN ? WG_K * 128 : WG_K * 2;
     constexpr uint32_t B_KSTEP = B_MN ? WG_K * 128 : WG_K * 2;
+    // main-loop turns: WG w waits on barrier 1 + w, the other WG arrives on it (2 x 128 threads)
+    const int my_turn_bar = 1 + wg, other_turn_bar = 2 - wg;
     uint32_t res_phase = 0;
     uint32_t out_it = 0;
-    uint32_t it = 0;
-    float acc[BLOCK_N / 2];
+    uint32_t it = 0;   // ring position; advances over the other WG's k-blocks too
+    float acc[2][BLOCK_N / 2];   // rows 0-63, rows 64-127 of the tile
 
-    for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
+    int j = 0;   // local tile index
+    for (int tile = first_tile; tile < total_tiles; tile += tile_step, ++j) {
       const int ks = tile % s.k_splits;
       const int t2 = tile / s.k_splits;
       const int n_blk = t2 % s.num_n_blocks;
       const int m_blk = t2 / s.num_n_blocks;
-      const int kb0 = (int)(((long long)ks * s.k_blocks) / s.k_splits);
-      const int kb1 = (int)(((long long)(ks + 1) * s.k_blocks) / s.k_splits);
-      const int row0 = m_blk * BLOCK_M + row_off;     // first row of this warp's slabs
+      const int kb0 = ks * s.k_blocks / s.k_splits;
+      const int kb1 = (ks + 1) * s.k_blocks / s.k_splits;
+      const int n_kb = (kb1 - kb0) * s.k_passes;
+      if ((j & 1) != wg) {   // the other WG's tile
+        it += n_kb;
+        continue;
+      }
       const int col_base = n_blk * BLOCK_N;
       // the tile's first residual slab travels while the main loop runs
       if (RES && lane == 0) {
         mbar_arrive_expect_tx(my_res_bar, SLAB_BYTES);
-        tma_load_2d(res_slab, &tmap_res, my_res_bar, col_base, row0);
+        tma_load_2d(res_slab, &tmap_res, my_res_bar, col_base, m_blk * BLOCK_M + row_off);
       }
 
-      const int n_kb = (kb1 - kb0) * s.k_passes;
+      // wait for the other WG to have issued the previous tile's main loop
+      if (j > 0) named_bar_sync(my_turn_bar, 256);
       uint32_t prev_stage = 0;
       for (int kbi = 0; kbi < n_kb; ++kbi, ++it) {
         const uint32_t stage = it % STAGES;
         const uint32_t ph = (it / STAGES) & 1u;
         mbar_wait(&full_bar[stage], ph);
-        const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES) + wg * 8192;
-        const uint32_t sb = smem_u32(smem + stage * Cfg::STAGE_BYTES) + Cfg::A_BYTES;
+        const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
+        const uint32_t sb = sa + Cfg::A_BYTES;
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BLOCK_K / WG_K; ++k)
-          wgmma_m64n128k16<A_MN, B_MN>(acc, make_sw128_desc(sa + k * A_KSTEP, A_LBO, 1024),
-                                       make_sw128_desc(sb + k * B_KSTEP, B_LBO, 1024),
-                                       (kbi > 0 || k > 0) ? 1u : 0u);
+        for (int k = 0; k < BLOCK_K / WG_K; ++k) {
+          const uint64_t bdesc = make_sw128_desc(sb + k * B_KSTEP, B_LBO, 1024);
+          const uint32_t scale_d = (kbi > 0 || k > 0) ? 1u : 0u;
+          wgmma_m64n128k16<A_MN, B_MN>(acc[0], make_sw128_desc(sa + k * A_KSTEP, A_LBO, 1024),
+                                       bdesc, scale_d);
+          wgmma_m64n128k16<A_MN, B_MN>(
+              acc[1], make_sw128_desc(sa + 8192 + k * A_KSTEP, A_LBO, 1024), bdesc, scale_d);
+        }
         wgmma_commit();
         // the previous k-block's MMAs have retired once at most this group is pending
         wgmma_wait<1>();
         if (kbi > 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
         prev_stage = stage;
       }
+      // every MMA of this tile is issued: the other WG's next tile may take the tensor cores
+      // (only if it has one, so that every arrive meets a sync)
+      if (tile + tile_step < total_tiles) named_bar_arrive(other_turn_bar, 256);
       wgmma_wait<0>();
-      wgmma_fence_acc(acc);
+      wgmma_fence_acc(acc[0]);
+      wgmma_fence_acc(acc[1]);
       if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
 
       // ------------------------------------------------------------- epilogue
-      const int ra = row0 + fr, rb = ra + 8;
-      const bool ra_ok = ra < s.M, rb_ok = rb < s.M;
-      int lab_a = -1, lab_b = -1;
-      float lse_a = 0.f, lse_b = 0.f, g_a = 0.f, g_b = 0.f;
-      if (ACT == ACT_CE || ACT == ACT_CE_GRAD) {
-        if (ra_ok) lab_a = __ldg(e.ce_label + ra);
-        if (rb_ok) lab_b = __ldg(e.ce_label + rb);
-        if (ACT == ACT_CE_GRAD) {
-          if (ra_ok) { lse_a = __ldg(e.ce_lse + ra); g_a = __ldg(e.ce_g + ra); }
-          if (rb_ok) { lse_b = __ldg(e.ce_lse + rb); g_b = __ldg(e.ce_g + rb); }
-        }
-      }
-      float lsc_a = 0.f, lsh_a = 0.f, lsc_b = 0.f, lsh_b = 0.f;   // (r - mean) * rstd
-      if (RES == RES_F32_LN) {
-        if (ra_ok) { lsc_a = __ldg(e.ln_rstd + ra); lsh_a = -__ldg(e.ln_mean + ra) * lsc_a; }
-        if (rb_ok) { lsc_b = __ldg(e.ln_rstd + rb); lsh_b = -__ldg(e.ln_mean + rb) * lsc_b; }
-      }
 #pragma unroll
-      for (int c = 0; c < NSLAB; ++c) {
-        const int col0 = col_base + c * W;
-        if (col0 >= s.N) break;  // warp-uniform
-        // v[4jj + 2h + x] = (row fr + 8h, column col0 + 8jj + fc + x)
-        float v[NV];
-#pragma unroll
-        for (int q = 0; q < NV; ++q) v[q] = acc[c * NV + q];
-        if (has_bias) {
-#pragma unroll
-          for (int jj = 0; jj < W / 8; ++jj) {
-            const int col = col0 + 8 * jj + fc;
-            if (col < s.N) {
-              const float2 b = __ldg(reinterpret_cast<const float2*>(e.bias + col));
-              v[4 * jj] += b.x; v[4 * jj + 1] += b.y; v[4 * jj + 2] += b.x; v[4 * jj + 3] += b.y;
-            }
+      for (int half = 0; half < 2; ++half) {
+        const int row0 = m_blk * BLOCK_M + half * 64 + row_off;   // first row of this warp's slabs
+        const int ra = row0 + fr, rb = ra + 8;
+        const bool ra_ok = ra < s.M, rb_ok = rb < s.M;
+        int lab_a = -1, lab_b = -1;
+        float lse_a = 0.f, lse_b = 0.f, g_a = 0.f, g_b = 0.f;
+        if (ACT == ACT_CE || ACT == ACT_CE_GRAD) {
+          if (ra_ok) lab_a = __ldg(e.ce_label + ra);
+          if (rb_ok) lab_b = __ldg(e.ce_label + rb);
+          if (ACT == ACT_CE_GRAD) {
+            if (ra_ok) { lse_a = __ldg(e.ce_lse + ra); g_a = __ldg(e.ce_g + ra); }
+            if (rb_ok) { lse_b = __ldg(e.ce_lse + rb); g_b = __ldg(e.ce_g + rb); }
           }
         }
-        // residual / saved-derivative slab (requested one slab ago) -> registers; its smem slab is
-        // then free for the next request
-        uint32_t opnd[NV];   // bf16 pairs (W = 64: NV / 2 used) or fp32 bits (W = 32)
-        if (RES) {
-          mbar_wait(my_res_bar, res_phase);
-          res_phase ^= 1u;
+        float lsc_a = 0.f, lsh_a = 0.f, lsc_b = 0.f, lsh_b = 0.f;   // (r - mean) * rstd
+        if (RES == RES_F32_LN) {
+          if (ra_ok) { lsc_a = __ldg(e.ln_rstd + ra); lsh_a = -__ldg(e.ln_mean + ra) * lsc_a; }
+          if (rb_ok) { lsc_b = __ldg(e.ln_rstd + rb); lsh_b = -__ldg(e.ln_mean + rb) * lsc_b; }
+        }
 #pragma unroll
-          for (int jj = 0; jj < W / 8; ++jj)
+        for (int c = 0; c < NSLAB; ++c) {
+          const int col0 = col_base + c * W;
+          if (col0 >= s.N) break;  // warp-uniform
+          // v[4jj + 2h + x] = (row fr + 8h, column col0 + 8jj + fc + x). The accumulator is
+          // cleared as it is read: the next tile's first MMA ignores it (scale-d 0), but to the
+          // compiler it is an input, and 128 live accumulators beside the epilogue would spill.
+          float v[NV];
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int r = fr + 8 * h;
-              if (W == 64) {
-                opnd[2 * jj + h] =
-                    *reinterpret_cast<const uint32_t*>(res_slab + slab_off(r, (8 * jj + fc) * 2));
-              } else {
-                const uint2 u =
-                    *reinterpret_cast<const uint2*>(res_slab + slab_off(r, (8 * jj + fc) * 4));
-                opnd[4 * jj + 2 * h] = u.x;
-                opnd[4 * jj + 2 * h + 1] = u.y;
+          for (int q = 0; q < NV; ++q) {
+            v[q] = acc[half][c * NV + q];
+            acc[half][c * NV + q] = 0.f;
+          }
+          if (has_bias) {
+#pragma unroll
+            for (int jj = 0; jj < W / 8; ++jj) {
+              const int col = col0 + 8 * jj + fc;
+              if (col < s.N) {
+                const float2 b = __ldg(reinterpret_cast<const float2*>(e.bias + col));
+                v[4 * jj] += b.x; v[4 * jj + 1] += b.y; v[4 * jj + 2] += b.x; v[4 * jj + 3] += b.y;
               }
             }
-          __syncwarp();
-          if (lane == 0 && c + 1 < NSLAB && col0 + W < s.N) {
-            mbar_arrive_expect_tx(my_res_bar, SLAB_BYTES);
-            tma_load_2d(res_slab, &tmap_res, my_res_bar, col0 + W, row0);
           }
-        }
-        // activation (compile-time); the training FFN-up also emits gelu'(x) through its own slab
-        if constexpr (ACT == ACT_GELU) {
-          if (has_aux) {
-            if (lane == 0) bulk_wait_read<1>();   // the aux slab's previous store (two groups back)
+          // residual / saved-derivative slab (requested one slab ago) -> registers; the next one is
+          // requested once these values have been used (below)
+          uint32_t opnd[NV];   // bf16 pairs (W = 64: NV / 2 used) or fp32 bits (W = 32)
+          if (RES) {
+            mbar_wait(my_res_bar, res_phase);
+            res_phase ^= 1u;
+#pragma unroll
+            for (int jj = 0; jj < W / 8; ++jj)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int r = fr + 8 * h;
+                if (W == 64) {
+                  opnd[2 * jj + h] =
+                      *reinterpret_cast<const uint32_t*>(res_slab + slab_off(r, (8 * jj + fc) * 2));
+                } else {
+                  const uint2 u =
+                      *reinterpret_cast<const uint2*>(res_slab + slab_off(r, (8 * jj + fc) * 4));
+                  opnd[4 * jj + 2 * h] = u.x;
+                  opnd[4 * jj + 2 * h + 1] = u.y;
+                }
+              }
+          }
+          // activation (compile-time); the training FFN-up also emits gelu'(x) through its own slab
+          if constexpr (ACT == ACT_GELU) {
+            if (has_aux) {
+              if (lane == 0) bulk_wait_read<1>();   // the aux slab's previous store (two groups back)
+              __syncwarp();
+#pragma unroll
+              for (int jj = 0; jj < W / 8; ++jj)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  float d0, d1;
+                  v[4 * jj + 2 * h] = gelu_erf_with_grad(v[4 * jj + 2 * h], d0);
+                  v[4 * jj + 2 * h + 1] = gelu_erf_with_grad(v[4 * jj + 2 * h + 1], d1);
+                  *reinterpret_cast<uint32_t*>(aux_slab + slab_off(fr + 8 * h, (8 * jj + fc) * 2)) =
+                      pack_bf16x2(d0, d1);
+                }
+              fence_proxy_async();
+              __syncwarp();
+              if (lane == 0) {
+                tma_store_2d(&tmap_aux, aux_slab, col0, row0);
+                bulk_commit();
+              }
+            } else {
+#pragma unroll
+              for (int q = 0; q < NV; ++q) v[q] = gelu_erf(v[q]);
+            }
+          } else if constexpr (ACT == ACT_RELU) {
+            if (has_aux) {   // pre-activation copy (the ReLU backward needs its sign)
+              if (lane == 0) bulk_wait_read<1>();
+              __syncwarp();
+#pragma unroll
+              for (int jj = 0; jj < W / 8; ++jj)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                  *reinterpret_cast<uint32_t*>(aux_slab + slab_off(fr + 8 * h, (8 * jj + fc) * 2)) =
+                      pack_bf16x2(v[4 * jj + 2 * h], v[4 * jj + 2 * h + 1]);
+              fence_proxy_async();
+              __syncwarp();
+              if (lane == 0) {
+                tma_store_2d(&tmap_aux, aux_slab, col0, row0);
+                bulk_commit();
+              }
+            }
+#pragma unroll
+            for (int q = 0; q < NV; ++q) v[q] = fmaxf(v[q], 0.0f);
+          } else if constexpr (ACT == ACT_CE) {
+            // online-softmax partials of each row over the slab's valid columns: the four lanes of a
+            // quad hold a row's columns
+            float m[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+            for (int jj = 0; jj < W / 8; ++jj)
+#pragma unroll
+              for (int x = 0; x < 2; ++x)
+                if (col0 + 8 * jj + fc + x < e.ce_n_valid) {
+                  m[0] = fmaxf(m[0], v[4 * jj + x]);
+                  m[1] = fmaxf(m[1], v[4 * jj + 2 + x]);
+                }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 1));
+              m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 2));
+            }
+            float ssum[2] = {0.f, 0.f};
+#pragma unroll
+            for (int jj = 0; jj < W / 8; ++jj)
+#pragma unroll
+              for (int x = 0; x < 2; ++x)
+                if (col0 + 8 * jj + fc + x < e.ce_n_valid) {
+                  ssum[0] += fast_ex2((v[4 * jj + x] - m[0]) * 1.4426950408889634f);
+                  ssum[1] += fast_ex2((v[4 * jj + 2 + x] - m[1]) * 1.4426950408889634f);
+                }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              ssum[h] += __shfl_xor_sync(0xffffffffu, ssum[h], 1);
+              ssum[h] += __shfl_xor_sync(0xffffffffu, ssum[h], 2);
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = h ? rb : ra;
+              if (!(h ? rb_ok : ra_ok)) continue;
+              if (fc == 0) e.ce_partial[(long long)(col0 / W) * e.ce_ld + row] = make_float2(m[h], ssum[h]);
+              const int rel = (h ? lab_b : lab_a) - col0;
+#pragma unroll
+              for (int jj = 0; jj < W / 8; ++jj)
+#pragma unroll
+                for (int x = 0; x < 2; ++x)
+                  if (rel == 8 * jj + fc + x) e.ce_lab[row] = v[4 * jj + 2 * h + x];
+            }
+          } else if constexpr (ACT == ACT_CE_GRAD) {
+#pragma unroll
+            for (int jj = 0; jj < W / 8; ++jj)
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int x = 0; x < 2; ++x) {
+                  const int j = 8 * jj + fc + x;
+                  const int q = 4 * jj + 2 * h + x;
+                  float p = fast_ex2((v[q] - (h ? lse_b : lse_a)) * 1.4426950408889634f);
+                  p = (j == (h ? lab_b : lab_a) - col0) ? p - 1.0f : p;
+                  v[q] = (col0 + j < e.ce_n_valid) ? p * (h ? g_b : g_a) : 0.f;
+                }
+          } else if constexpr (ACT == ACT_GELU_GRAD) {   // multiply by the saved activation derivative
+#pragma unroll
+            for (int jj = 0; jj < W / 8; ++jj)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const float2 x = unpack_bf16x2(opnd[2 * jj + h]);
+                v[4 * jj + 2 * h] *= x.x;
+                v[4 * jj + 2 * h + 1] *= x.y;
+              }
+          }
+          if (e.drop_threshold != 0u) {
+            // one hash per even/odd column pair: low half -> even, high half -> odd (dropout_keep)
+            const uint32_t t16 = e.drop_threshold >> 16;
+#pragma unroll
+            for (int jj = 0; jj < W / 8; ++jj)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const uint32_t idx = (uint32_t)(h ? rb : ra) * (uint32_t)s.N + (uint32_t)(col0 + 8 * jj + fc);
+                const uint32_t hh = hash_u32(e.drop_key, idx >> 1);
+                const int q = 4 * jj + 2 * h;
+                v[q] = ((hh & 0xFFFFu) >= t16) ? v[q] * e.drop_scale : 0.0f;
+                v[q + 1] = ((hh >> 16) >= t16) ? v[q + 1] * e.drop_scale : 0.0f;
+              }
+          }
+          if constexpr (RES == RES_F32) {
+#pragma unroll
+            for (int q = 0; q < NV; ++q) v[q] += __uint_as_float(opnd[q]);
+          } else if constexpr (RES == RES_F32_LN) {
+#pragma unroll
+            for (int jj = 0; jj < W / 8; ++jj) {
+              const int col = col0 + 8 * jj + fc;
+              float2 ga = make_float2(0.f, 0.f), be = make_float2(0.f, 0.f);
+              if (col < s.N) {
+                ga = __ldg(reinterpret_cast<const float2*>(e.ln_gamma + col));
+                be = __ldg(reinterpret_cast<const float2*>(e.ln_beta + col));
+              }
+              const int q = 4 * jj;
+              v[q] += fmaf(fmaf(__uint_as_float(opnd[q]), lsc_a, lsh_a), ga.x, be.x);
+              v[q + 1] += fmaf(fmaf(__uint_as_float(opnd[q + 1]), lsc_a, lsh_a), ga.y, be.y);
+              v[q + 2] += fmaf(fmaf(__uint_as_float(opnd[q + 2]), lsc_b, lsh_b), ga.x, be.x);
+              v[q + 3] += fmaf(fmaf(__uint_as_float(opnd[q + 3]), lsc_b, lsh_b), ga.y, be.y);
+            }
+          } else if constexpr (RES == RES_BF16 && ACT != ACT_GELU_GRAD) {
+#pragma unroll
+            for (int jj = 0; jj < W / 8; ++jj)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const float2 x = unpack_bf16x2(opnd[2 * jj + h]);
+                v[4 * jj + 2 * h] += x.x;
+                v[4 * jj + 2 * h + 1] += x.y;
+              }
+          }
+          if constexpr (OUT == OUT_NONE) {
+            // nothing to store
+          } else if constexpr (OUT == OUT_F32_ATOMIC) {
+#pragma unroll
+            for (int jj = 0; jj < W / 8; ++jj)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int col = col0 + 8 * jj + fc;
+                if ((h ? rb_ok : ra_ok) && col < s.N) {
+                  float* o = reinterpret_cast<float*>(e.out) + (long long)(h ? rb : ra) * e.ld_out + col;
+                  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(o),
+                               "f"(v[4 * jj + 2 * h]), "f"(v[4 * jj + 2 * h + 1])
+                               : "memory");
+                }
+              }
+          } else {
+            // stage the slab in swizzled smem and let TMA write full 128 B rows. Output slabs are
+            // double buffered: only the store issued two slabs ago must have finished READING smem
+            // (bulk groups complete in order; with an aux store per slab the distance is the same).
+            // (a GELU / ReLU kernel that stores no second tensor uses that tensor's slab as its
+            // second output buffer: the slabs are adjacent)
+            const bool two_bufs = (Cfg::N_OUT_BUF == 2) || (Cfg::AUX && !has_aux);
+            uint8_t* slab = out_slab + (two_bufs ? (out_it & 1u) * SLAB_BYTES : 0);
+            if (lane == 0) {
+              // one group may stay in flight when it reads another slab (the other output buffer,
+              // or this slab's derivative store); a lone slab must have drained
+              if (two_bufs || has_aux) bulk_wait_read<1>(); else bulk_wait_read<0>();
+            }
             __syncwarp();
 #pragma unroll
             for (int jj = 0; jj < W / 8; ++jj)
 #pragma unroll
               for (int h = 0; h < 2; ++h) {
-                float d0, d1;
-                v[4 * jj + 2 * h] = gelu_erf_with_grad(v[4 * jj + 2 * h], d0);
-                v[4 * jj + 2 * h + 1] = gelu_erf_with_grad(v[4 * jj + 2 * h + 1], d1);
-                *reinterpret_cast<uint32_t*>(aux_slab + slab_off(fr + 8 * h, (8 * jj + fc) * 2)) =
-                    pack_bf16x2(d0, d1);
+                const int r = fr + 8 * h, q = 4 * jj + 2 * h;
+                if (OUT == OUT_F32)
+                  *reinterpret_cast<float2*>(slab + slab_off(r, (8 * jj + fc) * 4)) =
+                      make_float2(v[q], v[q + 1]);
+                else
+                  *reinterpret_cast<uint32_t*>(slab + slab_off(r, (8 * jj + fc) * 2)) =
+                      pack_bf16x2(v[q], v[q + 1]);
               }
             fence_proxy_async();
             __syncwarp();
             if (lane == 0) {
-              tma_store_2d(&tmap_aux, aux_slab, col0, row0);
+              tma_store_2d(&tmap_out, slab, col0, row0);
               bulk_commit();
             }
-          } else {
-#pragma unroll
-            for (int q = 0; q < NV; ++q) v[q] = gelu_erf(v[q]);
-          }
-        } else if constexpr (ACT == ACT_RELU) {
-          if (has_aux) {   // pre-activation copy (the ReLU backward needs its sign)
-            if (lane == 0) bulk_wait_read<1>();
-            __syncwarp();
-#pragma unroll
-            for (int jj = 0; jj < W / 8; ++jj)
-#pragma unroll
-              for (int h = 0; h < 2; ++h)
-                *reinterpret_cast<uint32_t*>(aux_slab + slab_off(fr + 8 * h, (8 * jj + fc) * 2)) =
-                    pack_bf16x2(v[4 * jj + 2 * h], v[4 * jj + 2 * h + 1]);
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) {
-              tma_store_2d(&tmap_aux, aux_slab, col0, row0);
-              bulk_commit();
-            }
-          }
-#pragma unroll
-          for (int q = 0; q < NV; ++q) v[q] = fmaxf(v[q], 0.0f);
-        } else if constexpr (ACT == ACT_CE) {
-          // online-softmax partials of each row over the slab's valid columns: the four lanes of a
-          // quad hold a row's columns
-          float m[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-          for (int jj = 0; jj < W / 8; ++jj)
-#pragma unroll
-            for (int x = 0; x < 2; ++x)
-              if (col0 + 8 * jj + fc + x < e.ce_n_valid) {
-                m[0] = fmaxf(m[0], v[4 * jj + x]);
-                m[1] = fmaxf(m[1], v[4 * jj + 2 + x]);
-              }
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 1));
-            m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 2));
-          }
-          float ssum[2] = {0.f, 0.f};
-#pragma unroll
-          for (int jj = 0; jj < W / 8; ++jj)
-#pragma unroll
-            for (int x = 0; x < 2; ++x)
-              if (col0 + 8 * jj + fc + x < e.ce_n_valid) {
-                ssum[0] += fast_ex2((v[4 * jj + x] - m[0]) * 1.4426950408889634f);
-                ssum[1] += fast_ex2((v[4 * jj + 2 + x] - m[1]) * 1.4426950408889634f);
-              }
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            ssum[h] += __shfl_xor_sync(0xffffffffu, ssum[h], 1);
-            ssum[h] += __shfl_xor_sync(0xffffffffu, ssum[h], 2);
-          }
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int row = h ? rb : ra;
-            if (!(h ? rb_ok : ra_ok)) continue;
-            if (fc == 0) e.ce_partial[(long long)(col0 / W) * e.ce_ld + row] = make_float2(m[h], ssum[h]);
-            const int rel = (h ? lab_b : lab_a) - col0;
-#pragma unroll
-            for (int jj = 0; jj < W / 8; ++jj)
-#pragma unroll
-              for (int x = 0; x < 2; ++x)
-                if (rel == 8 * jj + fc + x) e.ce_lab[row] = v[4 * jj + 2 * h + x];
-          }
-        } else if constexpr (ACT == ACT_CE_GRAD) {
-#pragma unroll
-          for (int jj = 0; jj < W / 8; ++jj)
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-#pragma unroll
-              for (int x = 0; x < 2; ++x) {
-                const int j = 8 * jj + fc + x;
-                const int q = 4 * jj + 2 * h + x;
-                float p = fast_ex2((v[q] - (h ? lse_b : lse_a)) * 1.4426950408889634f);
-                p = (j == (h ? lab_b : lab_a) - col0) ? p - 1.0f : p;
-                v[q] = (col0 + j < e.ce_n_valid) ? p * (h ? g_b : g_a) : 0.f;
-              }
-        } else if constexpr (ACT == ACT_GELU_GRAD) {   // multiply by the saved activation derivative
-#pragma unroll
-          for (int jj = 0; jj < W / 8; ++jj)
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const float2 x = unpack_bf16x2(opnd[2 * jj + h]);
-              v[4 * jj + 2 * h] *= x.x;
-              v[4 * jj + 2 * h + 1] *= x.y;
-            }
-        }
-        if (e.drop_threshold != 0u) {
-          // one hash per even/odd column pair: low half -> even, high half -> odd (dropout_keep)
-          const uint32_t t16 = e.drop_threshold >> 16;
-#pragma unroll
-          for (int jj = 0; jj < W / 8; ++jj)
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const uint32_t idx = (uint32_t)(h ? rb : ra) * (uint32_t)s.N + (uint32_t)(col0 + 8 * jj + fc);
-              const uint32_t hh = hash_u32(e.drop_key, idx >> 1);
-              const int q = 4 * jj + 2 * h;
-              v[q] = ((hh & 0xFFFFu) >= t16) ? v[q] * e.drop_scale : 0.0f;
-              v[q + 1] = ((hh >> 16) >= t16) ? v[q + 1] * e.drop_scale : 0.0f;
-            }
-        }
-        if constexpr (RES == RES_F32) {
-#pragma unroll
-          for (int q = 0; q < NV; ++q) v[q] += __uint_as_float(opnd[q]);
-        } else if constexpr (RES == RES_F32_LN) {
-#pragma unroll
-          for (int jj = 0; jj < W / 8; ++jj) {
-            const int col = col0 + 8 * jj + fc;
-            float2 ga = make_float2(0.f, 0.f), be = make_float2(0.f, 0.f);
-            if (col < s.N) {
-              ga = __ldg(reinterpret_cast<const float2*>(e.ln_gamma + col));
-              be = __ldg(reinterpret_cast<const float2*>(e.ln_beta + col));
-            }
-            const int q = 4 * jj;
-            v[q] += fmaf(fmaf(__uint_as_float(opnd[q]), lsc_a, lsh_a), ga.x, be.x);
-            v[q + 1] += fmaf(fmaf(__uint_as_float(opnd[q + 1]), lsc_a, lsh_a), ga.y, be.y);
-            v[q + 2] += fmaf(fmaf(__uint_as_float(opnd[q + 2]), lsc_b, lsh_b), ga.x, be.x);
-            v[q + 3] += fmaf(fmaf(__uint_as_float(opnd[q + 3]), lsc_b, lsh_b), ga.y, be.y);
-          }
-        } else if constexpr (RES == RES_BF16 && ACT != ACT_GELU_GRAD) {
-#pragma unroll
-          for (int jj = 0; jj < W / 8; ++jj)
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const float2 x = unpack_bf16x2(opnd[2 * jj + h]);
-              v[4 * jj + 2 * h] += x.x;
-              v[4 * jj + 2 * h + 1] += x.y;
-            }
-        }
-        if constexpr (OUT == OUT_NONE) {
-          // nothing to store
-        } else if constexpr (OUT == OUT_F32_ATOMIC) {
-#pragma unroll
-          for (int jj = 0; jj < W / 8; ++jj)
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int col = col0 + 8 * jj + fc;
-              if ((h ? rb_ok : ra_ok) && col < s.N) {
-                float* o = reinterpret_cast<float*>(e.out) + (long long)(h ? rb : ra) * e.ld_out + col;
-                asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(o),
-                             "f"(v[4 * jj + 2 * h]), "f"(v[4 * jj + 2 * h + 1])
-                             : "memory");
+            // Every lane's residual values have now reached the slab just staged, so its reads of
+            // the residual slab are complete and TMA may refill it with the next slab: this
+            // half's next one, else the second half's first. (Issued right after the reads, the
+            // refill could overtake shared-memory loads held back behind the other warpgroup's
+            // MMA operand traffic.)
+            if (RES && lane == 0) {
+              if (c + 1 < NSLAB && col0 + W < s.N) {
+                mbar_arrive_expect_tx(my_res_bar, SLAB_BYTES);
+                tma_load_2d(res_slab, &tmap_res, my_res_bar, col0 + W, row0);
+              } else if (half == 0) {
+                mbar_arrive_expect_tx(my_res_bar, SLAB_BYTES);
+                tma_load_2d(res_slab, &tmap_res, my_res_bar, col_base, row0 + 64);
               }
             }
-        } else {
-          // stage the slab in swizzled smem and let TMA write full 128 B rows. Output slabs are
-          // double buffered: only the store issued two slabs ago must have finished READING smem
-          // (bulk groups complete in order; with an aux store per slab the distance is the same).
-          // (a GELU / ReLU kernel that stores no second tensor uses that tensor's slab as its
-          // second output buffer: the slabs are adjacent)
-          const bool two_bufs = (Cfg::N_OUT_BUF == 2) || (Cfg::AUX && !has_aux);
-          uint8_t* slab = out_slab + (two_bufs ? (out_it & 1u) * SLAB_BYTES : 0);
-          if (lane == 0) {
-            // one group may stay in flight when it reads another slab (the other output buffer,
-            // or this slab's derivative store); a lone slab must have drained
-            if (two_bufs || has_aux) bulk_wait_read<1>(); else bulk_wait_read<0>();
-          }
-          __syncwarp();
-#pragma unroll
-          for (int jj = 0; jj < W / 8; ++jj)
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int r = fr + 8 * h, q = 4 * jj + 2 * h;
-              if (OUT == OUT_F32)
-                *reinterpret_cast<float2*>(slab + slab_off(r, (8 * jj + fc) * 4)) =
-                    make_float2(v[q], v[q + 1]);
-              else
-                *reinterpret_cast<uint32_t*>(slab + slab_off(r, (8 * jj + fc) * 2)) =
-                    pack_bf16x2(v[q], v[q + 1]);
-            }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) {
-            tma_store_2d(&tmap_out, slab, col0, row0);
-            bulk_commit();
-          }
-          if constexpr (OUT == OUT_BF16 && W == 64) {
-            // column sums of the slab just staged (bf16, as stored): lane l owns columns
-            // 2l, 2l + 1 = word l of every 128-byte row (conflict-free), rows past M excluded
-            if (e.colsum != nullptr) {
-              const int rmax = min(SLAB_ROWS, s.M - row0);       // warp-uniform
-              float sx = 0.f, sy = 0.f;
-              const int u = lane >> 2, w4 = (lane & 3) * 4;
+            if constexpr (OUT == OUT_BF16 && W == 64) {
+              // column sums of the slab just staged (bf16, as stored): lane l owns columns
+              // 2l, 2l + 1 = word l of every 128-byte row (conflict-free), rows past M excluded
+              if (e.colsum != nullptr) {
+                const int rmax = min(SLAB_ROWS, s.M - row0);       // warp-uniform
+                float sx = 0.f, sy = 0.f;
+                const int u = lane >> 2, w4 = (lane & 3) * 4;
 #pragma unroll 8
-              for (int r = 0; r < rmax; ++r) {
-                const float2 x = unpack_bf16x2(
-                    *reinterpret_cast<const uint32_t*>(slab + r * 128 + ((u ^ (r & 7)) << 4) + w4));
-                sx += x.x;
-                sy += x.y;
+                for (int r = 0; r < rmax; ++r) {
+                  const float2 x = unpack_bf16x2(
+                      *reinterpret_cast<const uint32_t*>(slab + r * 128 + ((u ^ (r & 7)) << 4) + w4));
+                  sx += x.x;
+                  sy += x.y;
+                }
+                const int col = col0 + 2 * lane;
+                if (col < s.N && rmax > 0)
+                  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(e.colsum + col), "f"(sx),
+                               "f"(sy)
+                               : "memory");
               }
-              const int col = col0 + 2 * lane;
-              if (col < s.N && rmax > 0)
-                asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(e.colsum + col), "f"(sx),
-                             "f"(sy)
-                             : "memory");
             }
+            ++out_it;
           }
-          ++out_it;
         }
       }
     }
@@ -878,14 +924,18 @@ static int hero_gemm_bf16_impl(const hero_gemm_args* g, void* stream) {
     k_splits = 1;
   } else if (k_splits <= 0) {
     // Split K so that the (tiles x splits) work items fill whole waves of the resident CTAs:
-    // minimise  waves(s) * (k-blocks per split + epilogue)  over s. The epilogue of a
-    // split-K tile (128 x BLOCK_N fp32 atomics, not overlapped with anything when a CTA owns a
-    // single tile) costs about as much as 10 k-blocks of main loop. Keeps >= 4 k-blocks per
-    // split so the TMA pipeline has something to overlap; ties go to the smaller split count.
+    // minimise  waves(s) * (k-blocks per split + epi)  over s. epi is the cost of one more
+    // split-K work item (its 128 x BLOCK_N fp32 atomics into L2 and its pipeline fill) in
+    // k-blocks of main loop, fitted to CUDA-event timings of every split count at the four
+    // token-contracting weight gradients of the training step (768 x 3072, 3072 x 768,
+    // 2304 x 768, 768 x 768 at 16 512 tokens; H100 80GB HBM3, 700 W): any epi from 43 to 128
+    // picks the fastest or within 3 % of the fastest split there (2, 2, 1, 3), while the
+    // earlier epi = 10 picked 6, 6, 6, 7, up to 50 % slower. Keeps >= 4 k-blocks per split so
+    // the TMA pipeline has something to overlap; ties go to the smaller split count.
     const int tiles = s.num_m_blocks * s.num_n_blocks;
     const int slots = sms;   // concurrently resident tiles
     const int max_s = s.k_blocks / 4 > 1 ? s.k_blocks / 4 : 1;
-    const int epi = 10;
+    const int epi = 64;
     long long best_cost = -1;
     k_splits = 1;
     for (int sp = 1; sp <= max_s && sp <= 64; ++sp) {
@@ -898,6 +948,9 @@ static int hero_gemm_bf16_impl(const hero_gemm_args* g, void* stream) {
     }
   }
   if (k_splits > s.k_blocks) k_splits = s.k_blocks;
+  // the kernels split the k-blocks in 32-bit arithmetic (a 64-bit division is a subroutine call,
+  // and the registers live across it spill)
+  HERO_REQUIRE((long long)k_splits * s.k_blocks < (1ll << 31), "k_splits x k-blocks overflows");
   s.k_splits = k_splits;
   HERO_REQUIRE((g->a_lo == nullptr) == (g->b_lo == nullptr), "a_lo and b_lo go together");
   s.k_passes = g->a_lo ? 3 : 1;
