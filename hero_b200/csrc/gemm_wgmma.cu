@@ -22,6 +22,15 @@
 // Pipeline: smem full/empty ring (TMA <-> MMA); each stage is consumed by the one WG that owns
 // its tile. The producer runs ahead into the next tile while a consumer runs its epilogue.
 //
+// Wide form (BN = 256, the long-K GEMMs): 128 x 256 tiles, cooperative consumers. Both WGs take
+// every tile; WG w issues one wgmma.m64n256k16 per k16 step into rows 64w..64w+63 (again 128
+// accumulators per thread), so both read the same stage (empty barrier: 8 warp arrivals) and no
+// turn-taking is needed. The epilogue is the same per-slab code over the warp's 16 rows x 256
+// columns. Per 64-deep k-block the SM's shared memory then carries 48 KB of TMA writes and 80 KB
+// of operand reads for 1 024 tensor-core cycles (128 B/clk), against 32 KB + 48 KB for 512 cycles
+// (160 B/clk) with two m64n128k16 per step; but the tensor cores idle through the epilogue, which
+// only pays where the main loop is long (DESIGN §4, "Two tilings").
+//
 // Replaces the cuBLAS calls behind nn.Linear in model/layers.py:125-127,176,237,251,
 // model/embed.py:112 and model/layers.py:82-90 (reference), forward and backward.
 #include <cuda.h>
@@ -38,8 +47,9 @@
 namespace hero {
 
 constexpr int BLOCK_M = 128;
-// A consumer thread holds the whole 128 x 128 tile's fragment (128 fp32 accumulators) beside the
-// fused epilogue's working set within its 232 registers.
+// Tile width of the ping-pong form. A consumer thread holds the whole 128 x 128 tile's fragment
+// (128 fp32 accumulators) beside the fused epilogue's working set within its 232 registers; in
+// the wide form (BN = 256) the same 128 accumulators hold a 64 x 256 half tile.
 constexpr int BLOCK_N = 128;
 constexpr int BLOCK_K = 64;   // 64 bf16 = 128 bytes = one swizzle span
 constexpr int WG_K = 16;      // K of one wgmma
@@ -94,10 +104,11 @@ struct GemmEpilogue {
   float drop_scale;
 };
 
-template <int ACT, int OUT, int RES>
+template <int ACT, int OUT, int RES, int BN>
 struct GemmCfg {
+  static_assert(BN == BLOCK_N || BN == 256, "tiles are 128 x 128 (ping-pong) or 128 x 256 (wide)");
   static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
-  static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
+  static constexpr int B_BYTES = BN * BLOCK_K * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   // slab width in columns: 128-byte rows of the element type that travels
   static constexpr int W = (OUT == OUT_F32 || RES == RES_F32 || RES == RES_F32_LN) ? 32 : 64;
@@ -129,7 +140,7 @@ __device__ __forceinline__ uint32_t slab_off(int r, int b) {
   return r * 128 + ((((b >> 4) ^ (r & 7))) << 4) + (b & 15);
 }
 
-template <int A_MN, int B_MN, int ACT, int OUT, int RES>
+template <int A_MN, int B_MN, int ACT, int OUT, int RES, int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
                   const __grid_constant__ CUtensorMap tmap_b,
@@ -139,11 +150,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
                   const __grid_constant__ CUtensorMap tmap_a_lo,
                   const __grid_constant__ CUtensorMap tmap_b_lo, const GemmShape s,
                   const GemmEpilogue e) {
-  using Cfg = GemmCfg<ACT, OUT, RES>;
+  using Cfg = GemmCfg<ACT, OUT, RES, BN>;
+  constexpr bool WIDE = (BN == 256);
   constexpr int STAGES = Cfg::STAGES;
   constexpr int W = Cfg::W;
-  constexpr int NSLAB = BLOCK_N / W;
+  constexpr int NSLAB = BN / W;
   constexpr int NV = W / 2;   // fragment values of one slab per thread
+  // 64-row halves of a tile that one consumer WG holds: the whole tile (ping-pong), or its own
+  // half (wide: WG w owns rows 64w..64w+63)
+  constexpr int NHALF = WIDE ? 1 : 2;
   static_assert(!(ACT == ACT_GELU || ACT == ACT_RELU || ACT == ACT_GELU_GRAD) || W == 64,
                 "activation epilogues use 64-column bf16 slabs");
   static_assert(ACT != ACT_GELU_GRAD || RES == RES_BF16, "GELU' multiplier arrives as a bf16 slab");
@@ -169,7 +184,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
     if (RES) tma_prefetch_desc(&tmap_res);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 4);   // one arrive per warp of the consumer WG that owns the tile
+      // one arrive per warp of the consumer WG that owns the tile (wide: of both WGs)
+      mbar_init(&empty_bar[i], WIDE ? 8 : 4);
     }
     for (int i = 0; i < NUM_EPI_WARPS; ++i) mbar_init(&res_bar[i], 1);
     fence_barrier_init();
@@ -212,9 +228,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
             else
               tma_load_2d(sa, ma, &full_bar[stage], kb * BLOCK_K, m_blk * BLOCK_M);
             if (B_MN)
-              tma_load_3d(sb, mb, &full_bar[stage], 0, kb * BLOCK_K, n_blk * (BLOCK_N / 64));
+              tma_load_3d(sb, mb, &full_bar[stage], 0, kb * BLOCK_K, n_blk * (BN / 64));
             else
-              tma_load_2d(sb, mb, &full_bar[stage], kb * BLOCK_K, n_blk * BLOCK_N);
+              tma_load_2d(sb, mb, &full_bar[stage], kb * BLOCK_K, n_blk * BN);
           }
         }
       }
@@ -224,7 +240,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
     setmaxnreg_inc<CONSUMER_REGS>();
     const int cw = warp - 4;            // consumer warp 0..7: staging slabs, residual mbarrier
     const int wg = cw >> 2;             // 0 = WG1, 1 = WG2
-    const int row_off = (cw & 3) * SLAB_ROWS;   // this warp's 16 rows in each 64-row half
+    // this warp's 16 rows in each 64-row half the WG holds, from the tile's first row
+    const int row_off = (WIDE ? wg * 64 : 0) + (cw & 3) * SLAB_ROWS;
     const int fr = lane >> 2;          // fragment rows fr, fr + 8 of the warp's 16
     const int fc = (lane & 3) * 2;     // fragment columns 8j + fc, 8j + fc + 1
     uint8_t* stage0 = smem + Cfg::STAGING_OFFSET + cw * Cfg::SLABS_PER_WARP * SLAB_BYTES;
@@ -236,7 +253,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
     const bool has_bias = (e.bias != nullptr);
     // K-major: 8-row groups 1024 B apart (SBO), LBO unused (encoded 1).
     // MN-major: 64-element MN chunks BLOCK_K*128 B apart (LBO), 8-k groups 1024 B apart (SBO).
-    // Rows 64..127 of A start 8 KB into the stage in both layouts.
+    // Rows 64..127 of A start 8 KB into the stage in both layouts; so do columns 64.. of B, and
+    // an N = 256 wgmma reads all four 64-column chunks through the same descriptor.
     constexpr uint32_t A_LBO = A_MN ? BLOCK_K * 128 : 16;
     constexpr uint32_t B_LBO = B_MN ? BLOCK_K * 128 : 16;
     constexpr uint32_t A_KSTEP = A_MN ? WG_K * 128 : WG_K * 2;
@@ -246,7 +264,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
     uint32_t res_phase = 0;
     uint32_t out_it = 0;
     uint32_t it = 0;   // ring position; advances over the other WG's k-blocks too
-    float acc[2][BLOCK_N / 2];   // rows 0-63, rows 64-127 of the tile
+    float acc[NHALF][BN / 2];   // ping-pong: rows 0-63, rows 64-127 of the tile; wide: own half
 
     int j = 0;   // local tile index
     for (int tile = first_tile; tile < total_tiles; tile += tile_step, ++j) {
@@ -257,11 +275,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
       const int kb0 = ks * s.k_blocks / s.k_splits;
       const int kb1 = (ks + 1) * s.k_blocks / s.k_splits;
       const int n_kb = (kb1 - kb0) * s.k_passes;
-      if ((j & 1) != wg) {   // the other WG's tile
+      if (!WIDE && (j & 1) != wg) {   // the other WG's tile
         it += n_kb;
         continue;
       }
-      const int col_base = n_blk * BLOCK_N;
+      const int col_base = n_blk * BN;
       // the tile's first residual slab travels while the main loop runs
       if (RES && lane == 0) {
         mbar_arrive_expect_tx(my_res_bar, SLAB_BYTES);
@@ -269,7 +287,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
       }
 
       // wait for the other WG to have issued the previous tile's main loop
-      if (j > 0) named_bar_sync(my_turn_bar, 256);
+      if (!WIDE && j > 0) named_bar_sync(my_turn_bar, 256);
       uint32_t prev_stage = 0;
       for (int kbi = 0; kbi < n_kb; ++kbi, ++it) {
         const uint32_t stage = it % STAGES;
@@ -282,10 +300,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
         for (int k = 0; k < BLOCK_K / WG_K; ++k) {
           const uint64_t bdesc = make_sw128_desc(sb + k * B_KSTEP, B_LBO, 1024);
           const uint32_t scale_d = (kbi > 0 || k > 0) ? 1u : 0u;
-          wgmma_m64n128k16<A_MN, B_MN>(acc[0], make_sw128_desc(sa + k * A_KSTEP, A_LBO, 1024),
-                                       bdesc, scale_d);
-          wgmma_m64n128k16<A_MN, B_MN>(
-              acc[1], make_sw128_desc(sa + 8192 + k * A_KSTEP, A_LBO, 1024), bdesc, scale_d);
+          if constexpr (WIDE) {
+            wgmma_m64n256k16<A_MN, B_MN>(
+                acc[0], make_sw128_desc(sa + wg * 8192 + k * A_KSTEP, A_LBO, 1024), bdesc, scale_d);
+          } else {
+            wgmma_m64n128k16<A_MN, B_MN>(acc[0], make_sw128_desc(sa + k * A_KSTEP, A_LBO, 1024),
+                                         bdesc, scale_d);
+            wgmma_m64n128k16<A_MN, B_MN>(
+                acc[1], make_sw128_desc(sa + 8192 + k * A_KSTEP, A_LBO, 1024), bdesc, scale_d);
+          }
         }
         wgmma_commit();
         // the previous k-block's MMAs have retired once at most this group is pending
@@ -295,15 +318,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
       }
       // every MMA of this tile is issued: the other WG's next tile may take the tensor cores
       // (only if it has one, so that every arrive meets a sync)
-      if (tile + tile_step < total_tiles) named_bar_arrive(other_turn_bar, 256);
+      if (!WIDE && tile + tile_step < total_tiles) named_bar_arrive(other_turn_bar, 256);
       wgmma_wait<0>();
-      wgmma_fence_acc(acc[0]);
-      wgmma_fence_acc(acc[1]);
+#pragma unroll
+      for (int half = 0; half < NHALF; ++half) wgmma_fence_acc(acc[half]);
       if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
 
       // ------------------------------------------------------------- epilogue
 #pragma unroll
-      for (int half = 0; half < 2; ++half) {
+      for (int half = 0; half < NHALF; ++half) {
         const int row0 = m_blk * BLOCK_M + half * 64 + row_off;   // first row of this warp's slabs
         const int ra = row0 + fr, rb = ra + 8;
         const bool ra_ok = ra < s.M, rb_ok = rb < s.M;
@@ -575,7 +598,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
               if (c + 1 < NSLAB && col0 + W < s.N) {
                 mbar_arrive_expect_tx(my_res_bar, SLAB_BYTES);
                 tma_load_2d(res_slab, &tmap_res, my_res_bar, col0 + W, row0);
-              } else if (half == 0) {
+              } else if (half + 1 < NHALF) {
                 mbar_arrive_expect_tx(my_res_bar, SLAB_BYTES);
                 tma_load_2d(res_slab, &tmap_res, my_res_bar, col_base, row0 + 64);
               }
@@ -719,11 +742,11 @@ struct GemmMaps {
   CUtensorMap a, b, out, aux, res, a_lo, b_lo;
 };
 
-template <int A_MN, int B_MN, int ACT, int OUT, int RES>
+template <int A_MN, int B_MN, int ACT, int OUT, int RES, int BN = BLOCK_N>
 static int launch(const GemmMaps& tm, const GemmShape& s, const GemmEpilogue& e,
                   cudaStream_t stream) {
-  using Cfg = GemmCfg<ACT, OUT, RES>;
-  auto kern = gemm_wgmma_kernel<A_MN, B_MN, ACT, OUT, RES>;
+  using Cfg = GemmCfg<ACT, OUT, RES, BN>;
+  auto kern = gemm_wgmma_kernel<A_MN, B_MN, ACT, OUT, RES, BN>;
   static bool attr_set = false;
   if (!attr_set) {
     HERO_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -747,21 +770,38 @@ static int launch(const GemmMaps& tm, const GemmShape& s, const GemmEpilogue& e,
   return HERO_OK;
 }
 
+// The variants with a wide (128 x 256) form: the weight gradients, the forward FFN-down / out-
+// projection into the fp32 residual stream, and the dgrads with a bf16 residual (FFN-up `da`, QKV
+// `dx`). Must agree with the `wide ?` choices in dispatch().
+static bool has_wide_form(const hero_gemm_args* g) {
+  const int layout = g->a_mn_major * 2 + g->b_mn_major;
+  if (g->out_f32_accumulate) return layout == 0 || layout == 3;
+  if (g->out_f32_store) return layout == 0 && g->act == ACT_NONE && g->resid != nullptr;
+  return layout == 1 && g->act == ACT_NONE && g->resid != nullptr;
+}
+
 static int dispatch(const hero_gemm_args* g, const GemmMaps& tm, const GemmShape& s,
-                    const GemmEpilogue& e, cudaStream_t st) {
+                    const GemmEpilogue& e, bool wide, cudaStream_t st) {
   const int layout = g->a_mn_major * 2 + g->b_mn_major;
   const bool res = g->resid != nullptr;
   if (g->out_f32_accumulate) {
-    if (layout == 3) return launch<1, 1, ACT_NONE, OUT_F32_ATOMIC, RES_NONE>(tm, s, e, st);
-    if (layout == 0) return launch<0, 0, ACT_NONE, OUT_F32_ATOMIC, RES_NONE>(tm, s, e, st);
+    if (layout == 3)
+      return wide ? launch<1, 1, ACT_NONE, OUT_F32_ATOMIC, RES_NONE, 256>(tm, s, e, st)
+                  : launch<1, 1, ACT_NONE, OUT_F32_ATOMIC, RES_NONE>(tm, s, e, st);
+    if (layout == 0)
+      return wide ? launch<0, 0, ACT_NONE, OUT_F32_ATOMIC, RES_NONE, 256>(tm, s, e, st)
+                  : launch<0, 0, ACT_NONE, OUT_F32_ATOMIC, RES_NONE>(tm, s, e, st);
     return set_error(HERO_ERR_INVALID, "fp32-accumulate supports layouts (0,0) and (1,1)");
   }
   if (g->out_f32_store) {
     // the residual stream: fp32 pre-LayerNorm sums (forward out-projection / FFN-down)
     if (layout == 0 && g->act == ACT_NONE) {
       if (res && g->resid_ln_mean)
-        return launch<0, 0, ACT_NONE, OUT_F32, RES_F32_LN>(tm, s, e, st);
-      if (res) return launch<0, 0, ACT_NONE, OUT_F32, RES_F32>(tm, s, e, st);
+        return wide ? launch<0, 0, ACT_NONE, OUT_F32, RES_F32_LN, 256>(tm, s, e, st)
+                    : launch<0, 0, ACT_NONE, OUT_F32, RES_F32_LN>(tm, s, e, st);
+      if (res)
+        return wide ? launch<0, 0, ACT_NONE, OUT_F32, RES_F32, 256>(tm, s, e, st)
+                    : launch<0, 0, ACT_NONE, OUT_F32, RES_F32>(tm, s, e, st);
       return launch<0, 0, ACT_NONE, OUT_F32, RES_NONE>(tm, s, e, st);
     }
     return set_error(HERO_ERR_INVALID, "fp32-store output supports layout (0,0), act 0 only");
@@ -788,7 +828,9 @@ static int dispatch(const hero_gemm_args* g, const GemmMaps& tm, const GemmShape
   } else if (layout == 1) {
     switch (g->act) {
       case ACT_NONE:
-        if (res) return launch<0, 1, ACT_NONE, OUT_BF16, RES_BF16>(tm, s, e, st);
+        if (res)
+          return wide ? launch<0, 1, ACT_NONE, OUT_BF16, RES_BF16, 256>(tm, s, e, st)
+                      : launch<0, 1, ACT_NONE, OUT_BF16, RES_BF16>(tm, s, e, st);
         return launch<0, 1, ACT_NONE, OUT_BF16, RES_NONE>(tm, s, e, st);
       case ACT_GELU_GRAD:
         return launch<0, 1, ACT_GELU_GRAD, OUT_BF16, RES_BF16>(tm, s, e, st);
@@ -804,7 +846,7 @@ static int dispatch(const hero_gemm_args* g, const GemmMaps& tm, const GemmShape
 // Optional per-launch timing (bench.py roofline): CUDA events on the launching stream around every
 // GEMM launch between hero_gemm_profile_begin() and hero_gemm_profile_end().
 struct GemmProfileRec {
-  int m, n, k, a_mn, b_mn, act, f32;
+  int m, n, k, a_mn, b_mn, act, f32, block_n;
 };
 struct GemmProfile {
   bool on = false;
@@ -836,7 +878,7 @@ extern "C" int hero_gemm_profile_end(double* ms, double* flops, int64_t* launche
   // HERO_GEMM_PROFILE_DUMP=<path>: per-launch CSV (shape, variant, ms) for tuning
   const char* path = getenv("HERO_GEMM_PROFILE_DUMP");
   FILE* f = path ? fopen(path, "w") : nullptr;
-  if (f) fprintf(f, "m,n,k,a_mn,b_mn,act,f32,ms\n");
+  if (f) fprintf(f, "m,n,k,a_mn,b_mn,act,f32,block_n,ms\n");
   for (size_t i = 0; i + 1 < g_prof.ev.size(); i += 2) {
     HERO_CUDA_CHECK(cudaEventSynchronize(g_prof.ev[i + 1]));
     float t = 0.f;
@@ -844,7 +886,8 @@ extern "C" int hero_gemm_profile_end(double* ms, double* flops, int64_t* launche
     total += t;
     if (f && i / 2 < g_prof.rec.size()) {
       const GemmProfileRec& r = g_prof.rec[i / 2];
-      fprintf(f, "%d,%d,%d,%d,%d,%d,%d,%.5f\n", r.m, r.n, r.k, r.a_mn, r.b_mn, r.act, r.f32, t);
+      fprintf(f, "%d,%d,%d,%d,%d,%d,%d,%d,%.5f\n", r.m, r.n, r.k, r.a_mn, r.b_mn, r.act, r.f32,
+              r.block_n, t);
     }
   }
   if (f) fclose(f);
@@ -856,11 +899,11 @@ extern "C" int hero_gemm_profile_end(double* ms, double* flops, int64_t* launche
   return HERO_OK;
 }
 
-static int hero_gemm_bf16_impl(const hero_gemm_args* g, void* stream);
+static int hero_gemm_bf16_impl(const hero_gemm_args* g, void* stream, int* bn_used);
 
 extern "C" int hero_gemm_bf16(const hero_gemm_args* g, void* stream) {
   using namespace hero;
-  if (!g_prof.on) return hero_gemm_bf16_impl(g, stream);
+  if (!g_prof.on) return hero_gemm_bf16_impl(g, stream, nullptr);
   cudaEvent_t ev[2];
   for (int i = 0; i < 2; ++i) {
     if (!g_prof.pool.empty()) {
@@ -872,19 +915,20 @@ extern "C" int hero_gemm_bf16(const hero_gemm_args* g, void* stream) {
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   HERO_CUDA_CHECK(cudaEventRecord(ev[0], st));
-  const int rc = hero_gemm_bf16_impl(g, stream);
+  int bn = 0;
+  const int rc = hero_gemm_bf16_impl(g, stream, &bn);
   HERO_CUDA_CHECK(cudaEventRecord(ev[1], st));
   g_prof.ev.push_back(ev[0]);
   g_prof.ev.push_back(ev[1]);
   if (g)
     g_prof.rec.push_back(GemmProfileRec{g->m, g->n, g->k, g->a_mn_major, g->b_mn_major, g->act,
-                                        g->out_f32_accumulate + 2 * g->out_f32_store});
+                                        g->out_f32_accumulate + 2 * g->out_f32_store, bn});
   // (a split-bf16 GEMM issues 3x the MMAs; the profile counts its algorithmic 2MNK once)
   if (rc == HERO_OK && g) g_prof.flops += 2.0 * (double)g->m * (double)g->n * (double)g->k;
   return rc;
 }
 
-static int hero_gemm_bf16_impl(const hero_gemm_args* g, void* stream) {
+static int hero_gemm_bf16_impl(const hero_gemm_args* g, void* stream, int* bn_used) {
   using namespace hero;
   HERO_REQUIRE(g != nullptr, "null args");
   HERO_REQUIRE(g->a && g->b && (g->out || g->act == ACT_CE), "null operand pointer");
@@ -906,48 +950,67 @@ static int hero_gemm_bf16_impl(const hero_gemm_args* g, void* stream) {
                  (long long)g->lda);
   if (g->b_mn_major) HERO_REQUIRE(g->n % 64 == 0, "MN-major B needs n %% 64 == 0 (n=%d)", g->n);
 
-  // block_n 256 and cta_pair select Blackwell tilings (128 x 256 tiles, paired-CTA MMAs); on sm_90
-  // every GEMM runs on 128 x 128 tiles of one CTA, which compute the same result.
+  // block_n 128 runs the ping-pong 128 x 128 kernel, 256 the wide 128 x 256 one where the variant
+  // has a wide form (else 128 x 128), 0 picks per shape. cta_pair (a Blackwell tiling) is accepted
+  // and ignored.
   HERO_REQUIRE(g->block_n == 0 || g->block_n == 128 || g->block_n == 256,
                "block_n must be 0, 128 or 256");
   const int sms = sm_count();
   if (sms <= 0) return set_error(HERO_ERR_NO_DEVICE, "no CUDA device");
-  const int m_blocks = ceil_div(g->m, BLOCK_M);
 
   GemmShape s;
   s.M = g->m; s.N = g->n; s.K = g->k;
-  s.num_m_blocks = m_blocks;
-  s.num_n_blocks = ceil_div(g->n, BLOCK_N);
+  s.num_m_blocks = ceil_div(g->m, BLOCK_M);
   s.k_blocks = ceil_div(g->k, BLOCK_K);
-  int k_splits = g->k_splits;
-  if (!g->out_f32_accumulate) {
-    k_splits = 1;
-  } else if (k_splits <= 0) {
-    // Split K so that the (tiles x splits) work items fill whole waves of the resident CTAs:
-    // minimise  waves(s) * (k-blocks per split + epi)  over s. epi is the cost of one more
-    // split-K work item (its 128 x BLOCK_N fp32 atomics into L2 and its pipeline fill) in
-    // k-blocks of main loop, fitted to CUDA-event timings of every split count at the four
-    // token-contracting weight gradients of the training step (768 x 3072, 3072 x 768,
-    // 2304 x 768, 768 x 768 at 16 512 tokens; H100 80GB HBM3, 700 W): any epi from 43 to 128
-    // picks the fastest or within 3 % of the fastest split there (2, 2, 1, 3), while the
-    // earlier epi = 10 picked 6, 6, 6, 7, up to 50 % slower. Keeps >= 4 k-blocks per split so
-    // the TMA pipeline has something to overlap; ties go to the smaller split count.
-    const int tiles = s.num_m_blocks * s.num_n_blocks;
-    const int slots = sms;   // concurrently resident tiles
-    const int max_s = s.k_blocks / 4 > 1 ? s.k_blocks / 4 : 1;
-    const int epi = 64;
-    long long best_cost = -1;
-    k_splits = 1;
-    for (int sp = 1; sp <= max_s && sp <= 64; ++sp) {
-      const long long waves = ceil_div(tiles * sp, slots);
-      const long long cost = waves * (ceil_div(s.k_blocks, sp) + epi);
-      if (best_cost < 0 || cost < best_cost) {
+  // Tiling and split-K count minimise a cost in units of one 64-deep k-block of a 128 x 128
+  // ping-pong tile:  waves * (k-blocks per work item * kb_cost + epi),  waves = the persistent
+  // grid's passes over (tiles x splits) work items. kb_cost is 1, or WIDE_KB for the twice-as-wide
+  // tile; epi is what a work item's epilogue adds to its main loop. The ping-pong kernel hides a
+  // stored epilogue under the other warpgroup's MMAs (epi 0), the wide one does not (WIDE_EPI).
+  // A split-K item's fp32 atomics into L2 and pipeline fill cost SPLIT_EPI (x 2 for the wide
+  // tile's twice as many atomics); an fp32 stored tile has twice the slabs of a bf16 one and
+  // counts WIDE_EPI twice. Fitted to CUDA-event timings of both tilings (tools/gemm_probe.py) at
+  // the training step's shapes, 16 512 and 3 200 tokens, on an H100 80GB HBM3 at 700 W:
+  //   SPLIT_EPI = 64: any value from 43 to 128 picks the fastest 128 x 128 split, or one within
+  //   3 % of it, at the four 16 512-token weight gradients (768 x 3072, 3072 x 768, 2304 x 768,
+  //   768 x 768), where the earlier 10 picked splits up to 50 % slower.
+  //   WIDE_KB = 1.7, WIDE_EPI = 12 from the bf16-residual dgrads (K = 3072 and 2304: wide 3 %
+  //   faster and 1 % slower at 16 512 tokens). The wide split-K cost 2 x SPLIT_EPI (any value from
+  //   96 to 128) then picks, over all 17 probed GEMMs, a (tiling, split) within 5 % of the fastest,
+  //   and 128 x 256 for dW2 / dW1 (0.195 / 0.169 -> 0.157 / 0.137 ms) but not for dWqkv / dWo;
+  //   the fp32 LayerNorm-form FFN-down stays 128 x 128 (wide: 2 % slower at 16 512 tokens).
+  // Ties go to the 128 x 128 tiling and to the smaller split count; a split keeps >= 4 k-blocks so
+  // the TMA pipeline has something to overlap.
+  constexpr double WIDE_KB = 1.7, WIDE_EPI = 12.0, SPLIT_EPI = 64.0;
+  const bool wide_ok = has_wide_form(g);
+  double best_cost = -1.0;
+  int bn = BLOCK_N, k_splits = 1;
+  for (int cand = BLOCK_N; cand <= 256; cand *= 2) {
+    if (cand == 256 ? (!wide_ok || g->block_n == 128) : (wide_ok && g->block_n == 256)) continue;
+    const bool wide = (cand == 256);
+    const int tiles = s.num_m_blocks * ceil_div(g->n, cand);
+    int sp_lo = 1, sp_hi = 1;
+    if (g->out_f32_accumulate) {
+      if (g->k_splits > 0) {
+        sp_lo = sp_hi = g->k_splits < s.k_blocks ? g->k_splits : s.k_blocks;
+      } else {
+        sp_hi = s.k_blocks / 4 > 1 ? s.k_blocks / 4 : 1;
+        if (sp_hi > 64) sp_hi = 64;
+      }
+    }
+    const double epi = g->out_f32_accumulate ? SPLIT_EPI * (wide ? 2.0 : 1.0)
+                                             : (wide ? WIDE_EPI * (g->out_f32_store ? 2.0 : 1.0) : 0.0);
+    for (int sp = sp_lo; sp <= sp_hi; ++sp) {
+      const double waves = ceil_div(tiles * sp, sms);
+      const double cost = waves * (ceil_div(s.k_blocks, sp) * (wide ? WIDE_KB : 1.0) + epi);
+      if (best_cost < 0.0 || cost < best_cost) {
         best_cost = cost;
+        bn = cand;
         k_splits = sp;
       }
     }
   }
-  if (k_splits > s.k_blocks) k_splits = s.k_blocks;
+  s.num_n_blocks = ceil_div(g->n, bn);
   // the kernels split the k-blocks in 32-bit arithmetic (a 64-bit division is a subroutine call,
   // and the registers live across it spill)
   HERO_REQUIRE((long long)k_splits * s.k_blocks < (1ll << 31), "k_splits x k-blocks overflows");
@@ -999,9 +1062,9 @@ static int hero_gemm_bf16_impl(const hero_gemm_args* g, void* stream) {
     rc = get_tmap(&tm.a, g->a, g->m, g->k, g->lda, BLOCK_M, TM_KMAJOR);
   if (rc) return rc;
   if (g->b_mn_major)
-    rc = get_tmap(&tm.b, g->b, g->k, g->n, g->ldb, BLOCK_N, TM_MNMAJOR);
+    rc = get_tmap(&tm.b, g->b, g->k, g->n, g->ldb, bn, TM_MNMAJOR);
   else
-    rc = get_tmap(&tm.b, g->b, g->n, g->k, g->ldb, BLOCK_N, TM_KMAJOR);
+    rc = get_tmap(&tm.b, g->b, g->n, g->k, g->ldb, bn, TM_KMAJOR);
   if (rc) return rc;
   tm.a_lo = tm.a;
   tm.b_lo = tm.b;
@@ -1012,9 +1075,9 @@ static int hero_gemm_bf16_impl(const hero_gemm_args* g, void* stream) {
       rc = get_tmap(&tm.a_lo, g->a_lo, g->m, g->k, g->lda, BLOCK_M, TM_KMAJOR);
     if (rc) return rc;
     if (g->b_mn_major)
-      rc = get_tmap(&tm.b_lo, g->b_lo, g->k, g->n, g->ldb, BLOCK_N, TM_MNMAJOR);
+      rc = get_tmap(&tm.b_lo, g->b_lo, g->k, g->n, g->ldb, bn, TM_MNMAJOR);
     else
-      rc = get_tmap(&tm.b_lo, g->b_lo, g->n, g->k, g->ldb, BLOCK_N, TM_KMAJOR);
+      rc = get_tmap(&tm.b_lo, g->b_lo, g->n, g->k, g->ldb, bn, TM_KMAJOR);
     if (rc) return rc;
   }
   tm.out = tm.a;
@@ -1050,5 +1113,6 @@ static int hero_gemm_bf16_impl(const hero_gemm_args* g, void* stream) {
   }
 
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return dispatch(g, tm, s, e, st);
+  if (bn_used) *bn_used = bn;
+  return dispatch(g, tm, s, e, bn == 256, st);
 }

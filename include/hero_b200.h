@@ -98,7 +98,9 @@ typedef struct hero_gemm_args {
   uint32_t drop_threshold; /* 0 = no dropout; else p * 2^32 */
   uint32_t drop_key;
   float drop_scale;        /* 1 / (1 - p) */
-  int32_t block_n;         /* 0 = auto, 128 or 256; sm_90 runs every GEMM on 128 x 128 tiles */
+  int32_t block_n;         /* 0 = auto (per shape), 128 or 256 (128 x 256 tiles where the variant
+                              has a wide form: fp32 accumulate, fp32 store with a residual, bf16
+                              store with a bf16 residual and B MN-major; else 128 x 128) */
   int32_t k_splits;        /* 0 = auto (only > 1 when out_f32_accumulate) */
   int32_t cta_pair;        /* 0 = auto, 1 = single-CTA tiles, 2 = CTA pairs; sm_90 has no
                               paired-CTA MMA, so every value runs single-CTA tiles */
