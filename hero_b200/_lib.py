@@ -147,6 +147,10 @@ def _declare(lib):
     sig("hero_vsm_scores_bwd", vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp)
     sig("hero_vsm_span_fwd", vp, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp)
     sig("hero_vsm_span_bwd", vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp)
+    sig("hero_rank_topk", vp, i64, i32, i32, i32, f32, i32, vp, vp, vp)
+    sig("hero_vcmr_span_probs", vp, i64, vp, vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, vp, vp,
+        vp)
+    sig("hero_vcmr_moment_topn", vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp)
 
 
 def lib():

@@ -6,6 +6,11 @@
   `loader.BatchStager` ring (next batch's H2D copy and plan upload overlap the current forward) and
   the packed encoder runs without an autograd graph (activations ping-pong between two workspace
   slots, `hero_bert_stack_fwd` with save=False).
+* `VideoCorpus` / `rank_queries` / `full_vcmr_predictions` / `full_vr_predictions` — the ranking
+  half of eval_vcmr.py:205-418 and eval_vr.py:198-260: video scores, span probabilities and
+  moment lists of every query against the whole corpus, on the kernels of csrc/rank.cu (DESIGN §4
+  "Retrieval ranking"). No (Nq, K, L, L) tensor, no full sort, one small device->host copy per
+  query batch.
 * `ModelSaver` / `TrainingRestorer` — utils/save.py:112-181 with the same file layout (`vocab_padded`
   flag, `model_step_<n>.pt`, `train_state_<n>.pt`, `restore.pt` + backup), so checkpoints are
   interchangeable with the reference's; optimizer state is FusedAdamW's flat moments.
@@ -13,8 +18,10 @@
 import os
 from os.path import exists, join
 
+import numpy as np
 import torch
 
+from . import ops
 from .loader import BatchStager
 from .plan import PLAN_KEY, attach_plan
 
@@ -72,6 +79,360 @@ def embed_video_corpus(model, batches, n_videos, max_clip_len, device=None, vide
     if total is None:
         return None, None
     return total[:, :longest], masks[:, :longest]
+
+
+# ------------------------------------------------------------------ full-corpus ranking
+RANK_TASKS = ("VR", "VCMR", "SVMR")
+MAX_SELECT = 1024          # top-K clips and top-N moments per query (csrc/rank.cu)
+MAX_CLIP_LEN = 512         # frames per clip
+MAX_CORPUS = 65536         # clips per corpus
+# the fp32 query-vs-frame similarity block of one query chunk stays under this many bytes
+_S_BLOCK_BYTES = 256 << 20
+
+
+class VideoCorpus:
+    """A corpus prepared once for ranking: the frames of `embed_video_corpus` L2-normalised into
+    split-bf16 halves (the B operand of the similarity GEMM), their inverse norms (to recover the
+    raw dot products of the span head) and the frame mask as bytes.
+
+    frame_embeddings: (Nv, L, H) on the GPU; c_attn_masks: (Nv, L)."""
+
+    def __init__(self, frame_embeddings, c_attn_masks):
+        if frame_embeddings.dim() != 3 or tuple(c_attn_masks.shape) != frame_embeddings.shape[:2]:
+            raise ValueError(f"corpus of shape {tuple(frame_embeddings.shape)} with mask "
+                             f"{tuple(c_attn_masks.shape)}: expected (Nv, L, H) and (Nv, L)")
+        nv, length, d = frame_embeddings.shape
+        if not 1 <= length <= MAX_CLIP_LEN:
+            raise ValueError(f"clips of {length} frames: the ranking kernels take 1..{MAX_CLIP_LEN}")
+        if not 1 <= nv <= MAX_CORPUS:
+            raise ValueError(f"corpus of {nv} clips: the ranking kernels take 1..{MAX_CORPUS}")
+        if d % 8:
+            raise ValueError(f"hidden size {d} is not a multiple of 8")
+        dev = frame_embeddings.device
+        frames = frame_embeddings.float().contiguous().view(nv * length, d)
+        self.ld = (nv * length + 7) // 8 * 8              # GEMM N (and S row stride): multiple of 8
+        self.hi = torch.zeros((self.ld, d), dtype=torch.bfloat16, device=dev)
+        self.lo = torch.zeros((self.ld, d), dtype=torch.bfloat16, device=dev)
+        self.inv = torch.empty(nv * length, dtype=torch.float32, device=dev)
+        ops.l2norm_split(frames, self.hi, self.lo, self.inv)
+        self.mask = (c_attn_masks != 0).to(device=dev, dtype=torch.uint8).contiguous()
+        self.n_videos, self.length, self.dim, self.device = nv, length, d, dev
+
+
+def _check_rank_args(corpus, tasks, q2c_alpha, max_video, min_pred_l, max_pred_l, max_before_nms,
+                     gt_vidx, kernel_width):
+    tasks = tuple(tasks)
+    bad = [t for t in tasks if t not in RANK_TASKS]
+    if bad or not tasks:
+        raise ValueError(f"tasks {tasks}: expected a non-empty subset of {RANK_TASKS}")
+    if "VR" in tasks or "VCMR" in tasks:
+        if not 1 <= max_video <= min(MAX_SELECT, corpus.n_videos):
+            raise ValueError(f"max_video = {max_video}: needs 1 <= max_video <= "
+                             f"min({MAX_SELECT}, {corpus.n_videos} clips in the corpus)")
+    if "VCMR" in tasks:
+        if q2c_alpha is None or q2c_alpha <= 0:
+            raise ValueError("VCMR ranks exp(q2c_alpha * score): q2c_alpha must be > 0")
+        if max_video * corpus.length * corpus.length >= 1 << 31:
+            raise ValueError(f"max_video * L * L = {max_video * corpus.length ** 2} moments per "
+                             "query exceeds the kernel's 2^31 limit")
+    if "VCMR" in tasks or "SVMR" in tasks:
+        if not 1 <= max_before_nms <= MAX_SELECT:
+            raise ValueError(f"max_before_nms = {max_before_nms} outside [1, {MAX_SELECT}]")
+        if min_pred_l < 0:
+            raise ValueError(f"min_pred_l = {min_pred_l} < 0")
+        if kernel_width % 2 == 0 or kernel_width > 15:
+            raise ValueError(f"span convolution of width {kernel_width}: odd widths <= 15 only")
+    if "SVMR" in tasks:
+        if gt_vidx is None:
+            raise ValueError("SVMR needs gt_vidx, the ground-truth clip of every query")
+        if not (torch.is_tensor(gt_vidx) and gt_vidx.is_cuda):     # host values: checked here
+            g = np.asarray(gt_vidx.cpu() if torch.is_tensor(gt_vidx) else gt_vidx)
+            if g.size and (g.min() < 0 or g.max() >= corpus.n_videos):
+                raise ValueError(f"gt_vidx outside [0, {corpus.n_videos})")
+    return tasks
+
+
+@torch.no_grad()
+def rank_modularized(corpus, m, p, w_st, w_ed, *, tasks=RANK_TASKS, q2c_alpha=None, max_video=100,
+                     min_pred_l=2, max_pred_l=16, max_before_nms=200, gt_vidx=None):
+    """Ranking of encoded queries against a `VideoCorpus` (see `rank_queries`).
+
+    m: modularized queries (Nq, H); p = video_query_linear(m) (Nq, H), needed for VCMR / SVMR;
+    w_st / w_ed: the span convolution weights. Returns a dict of device tensors:
+      "VR":   (scores (Nq, K), clip rows (Nq, K) int32) — exp(q2c_alpha * s) when q2c_alpha is
+              given (eval_vcmr.py), s itself otherwise (eval_vr.py);
+      "VCMR": (scores (Nq, N), moments (Nq, N, 3) int32 = (clip row, start, end));
+      "SVMR": the same on each query's ground-truth clip.
+    Moments are ordered by descending score, ties to the lower flat index j*L*L + s*L + e; a query
+    with fewer than N band-valid spans is padded with score 0 and moments -1."""
+    kw = w_st.numel() if w_st is not None else 1
+    tasks = _check_rank_args(corpus, tasks, q2c_alpha, max_video, min_pred_l, max_pred_l,
+                             max_before_nms, gt_vidx, kw)
+    dev, nv, L, d = corpus.device, corpus.n_videos, corpus.length, corpus.dim
+    nq = m.shape[0]
+    need_v = "VR" in tasks or "VCMR" in tasks
+    need_p = "VCMR" in tasks or "SVMR" in tasks
+    if m.shape[1] != d or (need_p and tuple(p.shape) != tuple(m.shape)):
+        raise ValueError(f"queries of width {m.shape[1]} against a corpus of width {d}")
+    K, N = max_video, max_before_nms
+    f32, i32 = torch.float32, torch.int32
+    out = {}
+    if need_v:
+        v_val = torch.empty((nq, K), dtype=f32, device=dev)
+        v_idx = torch.empty((nq, K), dtype=i32, device=dev)
+        out["VR"] = (v_val, v_idx)
+    for t in ("VCMR", "SVMR"):
+        if t in tasks:
+            out[t] = (torch.empty((nq, N), dtype=f32, device=dev),
+                      torch.empty((nq, N, 3), dtype=i32, device=dev))
+    if nq == 0:
+        return out
+    m = m.float().contiguous()
+    if need_p:
+        p = p.float().contiguous()
+        ws = w_st.detach().float().reshape(-1).contiguous()
+        we = w_ed.detach().float().reshape(-1).contiguous()
+    if "SVMR" in tasks:
+        gt = torch.as_tensor(gt_vidx).to(device=dev, dtype=i32, non_blocking=True).reshape(nq)
+    # query chunks: [m^ ; p^] rows of one chunk x every corpus frame in fp32 <= _S_BLOCK_BYTES
+    rows_per_q = int(need_v) + int(need_p)
+    chunk = max(1, min(nq, _S_BLOCK_BYTES // (rows_per_q * corpus.ld * 4)))
+    for a in range(0, nq, chunk):
+        b = min(nq, a + chunk)
+        nc = b - a
+        n_rows = rows_per_q * nc
+        a_hi = torch.empty((n_rows, d), dtype=torch.bfloat16, device=dev)
+        a_lo = torch.empty_like(a_hi)
+        a_inv = torch.empty(n_rows, dtype=f32, device=dev)
+        r_p = nc if need_v else 0                            # first p^ row of the block
+        if need_v:
+            ops.l2norm_split(m[a:b], a_hi, a_lo, a_inv)
+        if need_p:
+            ops.l2norm_split(p[a:b], a_hi[r_p:], a_lo[r_p:], a_inv[r_p:])
+        s = torch.empty((n_rows, corpus.ld), dtype=f32, device=dev)
+        ops.gemm(a_hi, corpus.hi, s, a_lo=a_lo, b_lo=corpus.lo)
+        if need_v:
+            scores = torch.empty((nc, nv), dtype=f32, device=dev)
+            argmax = torch.empty((nc, nv), dtype=i32, device=dev)
+            ops.vsm_masked_max(s, corpus.mask, nc, nv, L, scores, argmax)
+            ops.rank_topk(scores, nv, K, v_val[a:b], v_idx[a:b],
+                          alpha=float(q2c_alpha or 0.0), apply_exp=q2c_alpha is not None)
+        if not need_p:
+            continue
+        q_rows = torch.arange(r_p, r_p + nc, dtype=i32, device=dev)
+        pr, pc = [], []
+        if "VCMR" in tasks:
+            pr.append(q_rows[:, None].expand(nc, K).reshape(-1))
+            pc.append(v_idx[a:b].reshape(-1))
+        if "SVMR" in tasks:
+            pr.append(q_rows)
+            pc.append(gt[a:b])
+        pair_row, pair_clip = torch.cat(pr), torch.cat(pc)
+        st = torch.empty((pair_row.numel(), L), dtype=f32, device=dev)
+        ed = torch.empty_like(st)
+        ops.vcmr_span_probs(s, pair_row, pair_clip, a_inv, corpus.inv, corpus.mask, ws, we, nv, L,
+                            st, ed)
+        off = 0
+        if "VCMR" in tasks:
+            score, mom = out["VCMR"]
+            ops.vcmr_moment_topn(st[:nc * K], ed[:nc * K], v_val[a:b], nc, K, L, min_pred_l,
+                                 max_pred_l, N, score[a:b], mom[a:b])
+            j = mom[a:b, :, 0]
+            clip = v_idx[a:b].gather(1, j.clamp(min=0).long())
+            mom[a:b, :, 0] = torch.where(j >= 0, clip, j)
+            off = nc * K
+        if "SVMR" in tasks:
+            score, mom = out["SVMR"]
+            ops.vcmr_moment_topn(st[off:], ed[off:], None, nc, 1, L, min_pred_l, max_pred_l, N,
+                                 score[a:b], mom[a:b])
+            j = mom[a:b, :, 0]
+            mom[a:b, :, 0] = torch.where(j >= 0, gt[a:b, None].expand_as(j), j)
+    return out
+
+
+@torch.no_grad()
+def rank_queries(model, corpus, query_batch, *, tasks=RANK_TASKS, q2c_alpha=None, max_video=100,
+                 min_pred_l=2, max_pred_l=16, max_before_nms=200, gt_vidx=None):
+    """Ranks one batch of queries against the whole corpus (eval_vcmr.py:232-323 and the SVMR
+    block of :326-354; eval_vr.py:223-233), without a host synchronisation.
+
+    query_batch: the reference's eval query batch on the GPU (`query_input_ids`, `query_pos_ids`,
+    `query_attn_masks`), with its text plan (plan.attach_plan(..., 'txt') on the host copy) under
+    plan.PLAN_KEY; without one the plan is built from the mask, which reads it back to the host.
+    The queries are encoded by the model's `encode_txt_inputs(..., attn_layer=q_feat_attn)`.
+    tasks: subset of ("VR", "VCMR", "SVMR"). See `rank_modularized` for the outputs.
+
+    Raises ValueError where the reference would fail or the kernels cannot go: max_video > Nv,
+    max_video or max_before_nms > 1024, L > 512, SVMR without gt_vidx.
+
+    Deviations from the reference (DESIGN §4 "Retrieval ranking"): ties are ordered
+    deterministically (descending score, lower index first) where torch.topk / torch.sort /
+    np.argsort leave them unspecified; only band-valid spans are listed (no zero-score filler)."""
+    m = model.encode_txt_inputs(query_batch["query_input_ids"], query_batch["query_pos_ids"],
+                                query_batch["query_attn_masks"], attn_layer=model.q_feat_attn,
+                                plan=query_batch.get(PLAN_KEY))
+    tasks = tuple(tasks)
+    p = None
+    if "VCMR" in tasks or "SVMR" in tasks:
+        p = model.video_query_linear(m.to(model.video_query_linear.weight.dtype))
+    return rank_modularized(corpus, m, p, model.video_st_predictor.weight,
+                            model.video_ed_predictor.weight, tasks=tasks, q2c_alpha=q2c_alpha,
+                            max_video=max_video, min_pred_l=min_pred_l, max_pred_l=max_pred_l,
+                            max_before_nms=max_before_nms, gt_vidx=gt_vidx)
+
+
+def _to_host(out):
+    """One device->host copy of every result tensor of a batch (bit-cast to int32 and packed)."""
+    keys = sorted(out)
+    parts, shapes = [], []
+    for k in keys:
+        for t in out[k]:
+            parts.append(t.reshape(-1).view(torch.int32) if t.dtype == torch.float32
+                         else t.reshape(-1))
+            shapes.append((t.shape, t.dtype))
+    flat = torch.cat(parts).cpu()
+    res, o = {}, 0
+    it = iter(shapes)
+    for k in keys:
+        vals = []
+        for _ in out[k]:
+            shape, dtype = next(it)
+            n = int(np.prod(shape))
+            v = flat[o:o + n]
+            o += n
+            vals.append((v.view(torch.float32) if dtype == torch.float32 else v).view(shape).numpy())
+        res[k] = tuple(vals)
+    return res
+
+
+class _QueryStager:
+    """Uploads each host query batch (tensors and text plan) on a side stream through a
+    `loader.BatchStager` ring; the current stream waits for the copy before the batch is ranked."""
+
+    def __init__(self, device):
+        self._ring = BatchStager(device, depth=2)
+        self._cur = torch.cuda.current_stream(device)
+        self._slot = None
+
+    def stage(self, host_batch):
+        (dev_batch,), ready, self._slot = self._ring.stage(host_batch)
+        self._cur.wait_event(ready)
+        return dev_batch
+
+    def release(self):
+        """After the work that reads the staged batch has been enqueued."""
+        self._ring.release(self._slot, self._cur)
+
+
+def _run_batches(model, corpus, batches, video_ids, rank_kw, want_gt):
+    """Encodes and ranks every query batch; returns (qids, per-batch host results, has_gt)."""
+    local = {vid: i for i, vid in enumerate(video_ids)}
+    stager = _QueryStager(corpus.device)
+    qids_all, results, has_gt = [], [], want_gt
+    was_training = model.training
+    model.eval()
+    for batch in batches:
+        hb = dict(batch)
+        qids, vids = hb.pop("qids"), hb.pop("vids")
+        targets = hb.pop("targets", None)
+        if has_gt and targets is not None and int(targets.min()) < 0:
+            has_gt = False                  # eval_vcmr.py:213-216: no GT -> predictions only
+        tasks = tuple(t for t in rank_kw["tasks"] if t != "SVMR" or has_gt)
+        qb = {k: hb[k] for k in ("query_input_ids", "query_pos_ids", "query_attn_masks")}
+        if "SVMR" in tasks:
+            qb["gt_vidx"] = torch.tensor([local[v] for v in vids], dtype=torch.int32)
+        tb = attach_plan({"input_ids": qb["query_input_ids"], "pos_ids": qb["query_pos_ids"],
+                          "attn_masks": qb["query_attn_masks"]}, "txt")
+        qb[PLAN_KEY] = tb[PLAN_KEY]             # built on the host: no read-back on the device
+        dqb = stager.stage(qb)
+        out = rank_queries(model, corpus, dqb, **dict(rank_kw, tasks=tasks),
+                           gt_vidx=dqb.get("gt_vidx"))
+        stager.release()
+        results.append(_to_host(out) if out else {})
+        qids_all.extend(qids)
+    if was_training:
+        model.train()
+    return qids_all, results, has_gt
+
+
+def _moment_records(score, mom, video_ids, video2idx, interval, svmr):
+    recs = []
+    keep = mom[:, 0] >= 0                     # padding past the last band-valid span
+    score, mom = score[keep], mom[keep]
+    if svmr:   # find_max_triples_from_upper_triangle_product + eval_vcmr.py:346-350 (float64)
+        st = mom[:, 1].astype(np.float64) * interval
+        ed = (mom[:, 2].astype(np.float64) + 1) * interval
+    else:      # eval_vcmr.py:396-400 (float32 frame indices)
+        st = mom[:, 1].astype(np.float32) * interval
+        ed = mom[:, 2].astype(np.float32) * interval + interval
+    for i in range(len(score)):
+        recs.append([video2idx[video_ids[int(mom[i, 0])]], float(st[i]), float(ed[i]),
+                     float(score[i])])
+    return recs
+
+
+def full_vcmr_predictions(model, corpus, batches, video_ids, video2idx, *, tasks=RANK_TASKS,
+                          q2c_alpha=20.0, max_vcmr_video=100, min_pred_l=2, max_pred_l=16,
+                          max_before_nms=200, vfeat_interval=1.5):
+    """The ranking half of the reference's full VCMR evaluation (eval_vcmr.py:205-418).
+
+    corpus: a `VideoCorpus` of the frames `embed_video_corpus` returned; batches: the reference's
+    full-eval query batches on the HOST (`vcmr_full_eval_collate`: qids, vids, targets and the
+    query tensors); video_ids: the clip id of every corpus row; video2idx: the global
+    id -> index map. Returns the reference's `eval_res` dict ({"SVMR", "VCMR", "VR"} lists of
+    `dict(desc_id, desc, predictions)`, empty ones dropped, plus "video2idx"), which its
+    `get_submission_top_n`, NMS and `eval_retrieval` consume unchanged.
+
+    As in the reference, VCMR is produced only together with VR, VR / VCMR only when the model
+    has a video-level loss weight, and SVMR only when every batch carries its targets. Flat VCMR
+    indices are decoded with the corpus's own L (the reference uses max_clip_len; the two agree
+    when the corpus holds a clip of max_clip_len frames); see `rank_queries` for the other stated
+    deviations."""
+    tasks = tuple(t for t in tasks if t in RANK_TASKS)
+    if model.lw_neg_ctx == 0 and model.lw_neg_q == 0:          # no q2video scores
+        tasks = tuple(t for t in tasks if t == "SVMR")
+    if "VR" not in tasks:                                       # VCMR reads the VR selection
+        tasks = tuple(t for t in tasks if t != "VCMR")
+    res = {"SVMR": [], "VCMR": [], "VR": []}
+    if tasks:
+        rank_kw = dict(tasks=tasks, q2c_alpha=q2c_alpha, max_video=max_vcmr_video,
+                       min_pred_l=min_pred_l, max_pred_l=max_pred_l, max_before_nms=max_before_nms)
+        qids, results, has_gt = _run_batches(model, corpus, batches, video_ids, rank_kw,
+                                             "SVMR" in tasks)
+        rows = [(r, i) for r in results for i in range(len(next(iter(r.values()))[0]))]
+        assert len(rows) == len(qids)
+        for qid, (r, i) in zip(qids, rows):
+            if "SVMR" in tasks and has_gt:
+                res["SVMR"].append(dict(desc_id=int(qid), desc="", predictions=_moment_records(
+                    *(x[i] for x in r["SVMR"]), video_ids, video2idx, vfeat_interval, True)))
+            if "VR" in r:
+                sc, ix = r["VR"][0][i][:100], r["VR"][1][i][:100]
+                res["VR"].append(dict(desc_id=int(qid), desc="", predictions=[
+                    [video2idx[video_ids[int(v)]], 0, 0, float(s)] for s, v in zip(sc, ix)]))
+            if "VCMR" in r:
+                res["VCMR"].append(dict(desc_id=int(qid), desc="", predictions=_moment_records(
+                    *(x[i] for x in r["VCMR"]), video_ids, video2idx, vfeat_interval, False)))
+    eval_res = {k: v for k, v in res.items() if len(v) != 0}
+    eval_res["video2idx"] = video2idx
+    return eval_res
+
+
+def full_vr_predictions(model, corpus, batches, video_ids, video2idx, *, max_vr_video=100):
+    """The ranking half of the reference's full video-retrieval evaluation (eval_vr.py:198-263):
+    the top `max_vr_video` clips of every query by its raw video score, the first 100 of them
+    listed as [video_idx, 0, 0, score]. Arguments and result as `full_vcmr_predictions`."""
+    rank_kw = dict(tasks=("VR",), q2c_alpha=None, max_video=max_vr_video)
+    qids, results, _ = _run_batches(model, corpus, batches, video_ids, rank_kw, False)
+    vr = []
+    rows = [(r, i) for r in results for i in range(len(r["VR"][0]))]
+    assert len(rows) == len(qids)
+    for qid, (r, i) in zip(qids, rows):
+        sc, ix = r["VR"][0][i][:100], r["VR"][1][i][:100]
+        vr.append(dict(desc_id=qid, desc="", predictions=[
+            [video2idx[video_ids[int(v)]], 0, 0, float(s)] for s, v in zip(sc, ix)]))
+    eval_res = {k: v for k, v in dict(VR=vr).items() if len(v) != 0}
+    eval_res["video2idx"] = video2idx
+    return eval_res
 
 
 class ModelSaver(object):

@@ -537,6 +537,51 @@ def vsm_span_bwd(dst, ded, mask_u8, w_st, w_ed, sim, query, ctx, dquery, dctx, d
 
 
 # ---------------------------------------------------------------------------------------------
+# Full-corpus retrieval ranking (hero_b200/csrc/rank.cu)
+def rank_topk(x, n, k, values, indices, alpha=0.0, apply_exp=False):
+    """values / indices [rows, k] = top-k of the first n columns of each row of x (fp32, row
+    stride x.stride(0)), descending, ties to the lower column; values are exp(alpha * x) when
+    apply_exp."""
+    _require_cuda(x, values, indices)
+    assert x.dtype == torch.float32 and x.stride(1) == 1
+    assert values.dtype == torch.float32 and indices.dtype == torch.int32
+    assert values.is_contiguous() and indices.is_contiguous()
+    _count()
+    _lib.check(_lib.lib().hero_rank_topk(_ptr(x), x.stride(0), x.shape[0], n, k, alpha,
+                                         int(apply_exp), _ptr(values), _ptr(indices), _stream()))
+
+
+def vcmr_span_probs(s, pair_row, pair_clip, row_inv, frame_inv, mask_u8, w_st, w_ed, nv, length,
+                    st, ed):
+    """st / ed [pairs, length] = start / end probabilities of the (row of s, clip) pairs."""
+    _require_cuda(s, pair_row, pair_clip, row_inv, frame_inv, mask_u8, st, ed)
+    assert s.dtype == torch.float32 and s.stride(1) == 1
+    for t in (pair_row, pair_clip):
+        assert t.dtype == torch.int32 and t.is_contiguous()
+    for t in (row_inv, frame_inv, w_st, w_ed, st, ed):
+        assert t.dtype == torch.float32 and t.is_contiguous()
+    assert mask_u8.dtype == torch.uint8 and mask_u8.is_contiguous()
+    _count()
+    _lib.check(_lib.lib().hero_vcmr_span_probs(
+        _ptr(s), s.stride(0), _ptr(pair_row), _ptr(pair_clip), pair_row.numel(), _ptr(row_inv),
+        _ptr(frame_inv), _ptr(mask_u8), _ptr(w_st), _ptr(w_ed), nv, length, w_st.numel(), _ptr(st),
+        _ptr(ed), _stream()))
+
+
+def vcmr_moment_topn(st, ed, video_factor, nq, k, length, min_l, max_l, n, score, jse):
+    """score [nq, n] / jse [nq, n, 3] = top-n band-valid moments of st[q, j, s] * factor[q, j] *
+    ed[q, j, e] per query (video_factor None: factor 1)."""
+    _require_cuda(st, ed, video_factor, score, jse)
+    for t in (st, ed, video_factor, score):
+        assert t is None or (t.dtype == torch.float32 and t.is_contiguous())
+    assert jse.dtype == torch.int32 and jse.is_contiguous()
+    _count()
+    _lib.check(_lib.lib().hero_vcmr_moment_topn(_ptr(st), _ptr(ed), _ptr(video_factor), nq, k,
+                                                length, min_l, max_l, n, _ptr(score), _ptr(jse),
+                                                _stream()))
+
+
+# ---------------------------------------------------------------------------------------------
 # Fused LM-head cross entropy (MLM): vocabulary logits are never materialised in fp32.
 def lm_head_ce_fwd(h, emb, bias, labels, n_valid):
     """h: bf16 [n, H] (LM-head transform of the masked tokens), emb: bf16 [V, H] (tied word

@@ -112,11 +112,15 @@ class HeroForPretraining(HeroModel):
 
     # ------------------------------------------------------------------ query side
     def encode_txt_inputs(self, input_ids, pos_ids, attn_masks, attn_layer=None,
-                          normalized=False):
+                          normalized=False, plan=None):
         """model/pretrain.py:168-186: text-only pass of the cross-modal transformer, optionally
-        L2-normalised, optionally pooled by `attn_layer` (the QueryFeatEncoder)."""
-        feats = self.v_encoder.f_encoder({"input_ids": input_ids, "pos_ids": pos_ids,
-                                          "attn_masks": attn_masks}, "txt")[0]
+        L2-normalised, optionally pooled by `attn_layer` (the QueryFeatEncoder). `plan`: the
+        batch's text plan built on the host (plan.attach_plan(..., 'txt')); without one it is built
+        from `attn_masks`, which reads a device mask back to the host."""
+        txt = {"input_ids": input_ids, "pos_ids": pos_ids, "attn_masks": attn_masks}
+        if plan is not None:
+            txt[PLAN_KEY] = plan
+        feats = self.v_encoder.f_encoder(txt, "txt")[0]
         if normalized:
             feats = F.normalize(feats, dim=-1, eps=1e-5)
         return feats if attn_layer is None else attn_layer(feats, attn_masks)
@@ -272,3 +276,40 @@ class HeroForVcmr(HeroForPretraining):
             q2video_scores = self.get_video_level_scores(modularized_query, frame_embeddings,
                                                          c_attn_masks, val_gather_gpus)
         return q2video_scores, st_prob, ed_prob
+
+
+class HeroForVr(HeroForVcmr):
+    """model/vr.py: MSR-VTT video retrieval (with or without subtitles) = the VCMR head with the
+    span loss off; trains on the video-level ranking losses only. Full-corpus ranking for its
+    evaluation is `evalpass.full_vr_predictions`."""
+
+    def __init__(self, config, vfeat_dim, max_frm_seq_len, ranking_loss_type="hinge", margin=0.1,
+                 lw_neg_ctx=1, lw_neg_q=1, use_hard_negative=False, hard_pool_size=20,
+                 hard_neg_weight=10, use_all_neg=True):
+        assert lw_neg_ctx != 0 or lw_neg_q != 0, \
+            "Need to set lw_neg_ctx or lw_neg_q for VR training"
+        super().__init__(config, vfeat_dim, max_frm_seq_len, ranking_loss_type=ranking_loss_type,
+                         margin=margin, lw_neg_ctx=lw_neg_ctx, lw_neg_q=lw_neg_q, lw_st_ed=0,
+                         drop_svmr_prob=1.0, use_hard_negative=use_hard_negative,
+                         hard_pool_size=hard_pool_size, hard_neg_weight=hard_neg_weight,
+                         use_all_neg=use_all_neg)
+        assert self.lw_st_ed == 0, "For VR, lw_st_ed should be 0"
+
+    def forward(self, batch, task="msrvtt_video_sub", compute_loss=True):
+        if task not in ("msrvtt_video_sub", "msrvtt_video_only"):
+            raise ValueError(f"Unrecognized task {task}")
+        if compute_loss:
+            _, loss_neg_ctx, loss_neg_q = super().forward(batch, task="tvr", compute_loss=True)
+            return loss_neg_ctx, loss_neg_q
+        q2video_scores, _, _ = super().forward(batch, task="tvr", compute_loss=False)
+        return q2video_scores
+
+    def get_pred_from_raw_query(self, frame_embeddings, c_attn_masks, query_input_ids,
+                                query_pos_ids, query_attn_masks, cross=False,
+                                val_gather_gpus=False):
+        """Video scores only (Nq, Nv), from unnormalised query features (model/vr.py:44-56)."""
+        modularized_query = self.encode_txt_inputs(query_input_ids, query_pos_ids,
+                                                   query_attn_masks, attn_layer=self.q_feat_attn,
+                                                   normalized=False)
+        return self.get_video_level_scores(modularized_query, frame_embeddings, c_attn_masks,
+                                           val_gather_gpus)

@@ -457,6 +457,33 @@ int hero_vsm_span_bwd(const float* dst, const float* ded, const uint8_t* mask, c
                       int32_t n, int32_t len, int32_t d, int32_t k, float* dquery, float* dctx,
                       float* dw_st, float* dw_ed, void* stream);
 
+/* ---- full-corpus retrieval ranking (hero_b200/csrc/rank.cu) ----
+ * Per-row top-k of x [rows, ld] over its first n columns (n <= 65536, k <= min(1024, n)), one CTA
+ * per row. values [rows, k] hold x (or exp(alpha * x) when apply_exp, alpha > 0, applied after
+ * the selection), indices [rows, k] the int32 columns. Order: descending value, ties to the
+ * lower column. */
+int hero_rank_topk(const float* x, int64_t ld, int32_t rows, int32_t n, int32_t k, float alpha,
+                   int32_t apply_exp, float* values, int32_t* indices, void* stream);
+/* Start / end probabilities of n_pairs (row, clip) pairs read from the output s [*, ld_s] of the
+ * p^ . c^ GEMM (column clip * len + l): sim[l] = s[row, clip * len + l] / (|row_inv[row]| *
+ * |frame_inv[clip * len + l]|) = p . c (inverse norms as hero_l2norm_split_f32 writes them; no
+ * zeroing at masked frames), then st / ed = softmax_l(mask_logits(conv1d_kw(sim), mask[clip])) with
+ * zero padding and no bias. st / ed are [n_pairs, len] fp32; a clip outside [0, nv) gives NaN.
+ * len <= 512, odd kw <= 15. */
+int hero_vcmr_span_probs(const float* s, int64_t ld_s, const int32_t* pair_row,
+                         const int32_t* pair_clip, int32_t n_pairs, const float* row_inv,
+                         const float* frame_inv, const uint8_t* mask, const float* w_st,
+                         const float* w_ed, int32_t nv, int32_t len, int32_t kw, float* st,
+                         float* ed, void* stream);
+/* Per query q (one CTA), the top n <= 1024 moments over its k clips j: score = st[q, j, s] *
+ * video_factor[q, j] * ed[q, j, e] (factor 1 when video_factor is NULL), over the band-valid spans
+ * min_l <= e - s < max_l, e < len only. st / ed [nq, k, len], video_factor [nq, k]. Outputs
+ * score [nq, n] and jse [nq, n, 3] = (j, s, e), descending score, ties to the lower j*len*len +
+ * s*len + e; when fewer than n spans exist the tail is score 0, jse -1. */
+int hero_vcmr_moment_topn(const float* st, const float* ed, const float* video_factor, int32_t nq,
+                          int32_t k, int32_t len, int32_t min_l, int32_t max_l, int32_t n,
+                          float* score, int32_t* jse, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
