@@ -151,6 +151,7 @@ def _declare(lib):
     sig("hero_vcmr_span_probs", vp, i64, vp, vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, vp, vp,
         vp)
     sig("hero_vcmr_moment_topn", vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp)
+    sig("hero_temporal_nms", vp, vp, i32, i32, i32, C.c_double, C.c_double, i32, i32, vp, vp, vp)
 
 
 def lib():

@@ -11,11 +11,16 @@
   moment lists of every query against the whole corpus, on the kernels of csrc/rank.cu (DESIGN §4
   "Retrieval ranking"). No (Nq, K, L, L) tensor, no full sort, one small device->host copy per
   query batch.
+* `nms_moments` / `eval_retrieval` / `full_vcmr_eval` — the rest of eval_vcmr.py:205-508:
+  temporal NMS of the ranked lists on the device (csrc/nms.cu), carried home in the same copy, and
+  the TVR recall metrics of utils/tvr_standalone_eval.py vectorised over queries on the host
+  (DESIGN §4 "Temporal NMS and TVR metrics").
 * `ModelSaver` / `TrainingRestorer` — utils/save.py:112-181 with the same file layout (`vocab_padded`
   flag, `model_step_<n>.pt`, `train_state_<n>.pt`, `restore.pt` + backup), so checkpoints are
   interchangeable with the reference's; optimizer state is FusedAdamW's flat moments.
 """
 import os
+from collections import OrderedDict
 from os.path import exists, join
 
 import numpy as np
@@ -324,8 +329,9 @@ class _QueryStager:
         self._ring.release(self._slot, self._cur)
 
 
-def _run_batches(model, corpus, batches, video_ids, rank_kw, want_gt):
-    """Encodes and ranks every query batch; returns (qids, per-batch host results, has_gt)."""
+def _run_batches(model, corpus, batches, video_ids, rank_kw, want_gt, post=None):
+    """Encodes and ranks every query batch; returns (qids, per-batch host results, has_gt).
+    `post(out)`, when given, maps each batch's device results to the dict that is copied."""
     local = {vid: i for i, vid in enumerate(video_ids)}
     stager = _QueryStager(corpus.device)
     qids_all, results, has_gt = [], [], want_gt
@@ -348,6 +354,8 @@ def _run_batches(model, corpus, batches, video_ids, rank_kw, want_gt):
         out = rank_queries(model, corpus, dqb, **dict(rank_kw, tasks=tasks),
                            gt_vidx=dqb.get("gt_vidx"))
         stager.release()
+        if post is not None:
+            out = post(out)
         results.append(_to_host(out) if out else {})
         qids_all.extend(qids)
     if was_training:
@@ -371,6 +379,15 @@ def _moment_records(score, mom, video_ids, video2idx, interval, svmr):
     return recs
 
 
+def _vcmr_tasks(model, tasks):
+    tasks = tuple(t for t in tasks if t in RANK_TASKS)
+    if model.lw_neg_ctx == 0 and model.lw_neg_q == 0:          # no q2video scores
+        tasks = tuple(t for t in tasks if t == "SVMR")
+    if "VR" not in tasks:                                       # VCMR reads the VR selection
+        tasks = tuple(t for t in tasks if t != "VCMR")
+    return tasks
+
+
 def full_vcmr_predictions(model, corpus, batches, video_ids, video2idx, *, tasks=RANK_TASKS,
                           q2c_alpha=20.0, max_vcmr_video=100, min_pred_l=2, max_pred_l=16,
                           max_before_nms=200, vfeat_interval=1.5):
@@ -388,11 +405,7 @@ def full_vcmr_predictions(model, corpus, batches, video_ids, video2idx, *, tasks
     indices are decoded with the corpus's own L (the reference uses max_clip_len; the two agree
     when the corpus holds a clip of max_clip_len frames); see `rank_queries` for the other stated
     deviations."""
-    tasks = tuple(t for t in tasks if t in RANK_TASKS)
-    if model.lw_neg_ctx == 0 and model.lw_neg_q == 0:          # no q2video scores
-        tasks = tuple(t for t in tasks if t == "SVMR")
-    if "VR" not in tasks:                                       # VCMR reads the VR selection
-        tasks = tuple(t for t in tasks if t != "VCMR")
+    tasks = _vcmr_tasks(model, tasks)
     res = {"SVMR": [], "VCMR": [], "VR": []}
     if tasks:
         rank_kw = dict(tasks=tasks, q2c_alpha=q2c_alpha, max_video=max_vcmr_video,
@@ -433,6 +446,288 @@ def full_vr_predictions(model, corpus, batches, video_ids, video2idx, *, max_vr_
     eval_res = {k: v for k, v in dict(VR=vr).items() if len(v) != 0}
     eval_res["video2idx"] = video2idx
     return eval_res
+
+
+# ------------------------------------------------------------------ temporal NMS and TVR metrics
+TVR_TASKS = ("VCMR", "SVMR", "VR")          # utils/tvr_standalone_eval.py TASK_TYPES order
+RECALL_TOPKS = (1, 5, 10, 100)
+MAX_PRED_PER_QUERY = 100
+DESC_TYPES = ("v", "t", "vt")
+
+
+def nms_moments(score, mom, *, nms_thd, n_in, n_out, interval, by_clip):
+    """Greedy temporal NMS of ranked moment lists on the device (csrc/nms.cu), with no host
+    synchronisation: the post-processing of post_processing_vcmr_nms (by_clip=True: per clip, then
+    merged by score) and post_processing_svmr_nms (by_clip=False: one list).
+
+    score (Nq, N) / mom (Nq, N, 3) as `rank_modularized` returns them (clip row, start, end frame;
+    descending score; padded with -1). Reads the first n_in entries of each row; spans are in
+    seconds of `interval` per frame, as the submission records them. An entry is dropped when its
+    IoU with a kept, higher-ranked entry of its group is > nms_thd; at most 100 are kept per group.
+    Returns (score (Nq, n_out), mom (Nq, n_out, 3)), padded with 0 / -1."""
+    if not 0 <= n_in <= min(MAX_SELECT, score.shape[1]):
+        raise ValueError(f"n_in = {n_in} outside [0, min({MAX_SELECT}, {score.shape[1]})]")
+    if not 1 <= n_out <= MAX_SELECT:
+        raise ValueError(f"n_out = {n_out} outside [1, {MAX_SELECT}]")
+    nq, dev = score.shape[0], score.device
+    out_s = torch.empty((nq, n_out), dtype=torch.float32, device=dev)
+    out_m = torch.empty((nq, n_out, 3), dtype=torch.int32, device=dev)
+    ops.temporal_nms(score, mom, n_in, nms_thd, interval, by_clip, n_out, out_s, out_m)
+    return out_s, out_m
+
+
+def _rounded_percentage(x):
+    return round(x * 100, 2)                  # get_rounded_percentage
+
+
+def _pack_lists(lists):
+    """Per-query prediction lists -> (vid, st, ed) float32 (n, P) and valid (n, P), the first
+    MAX_PRED_PER_QUERY entries of each, as eval_by_task_type reads them."""
+    rows = [p[:MAX_PRED_PER_QUERY] for p in lists]
+    lens = np.fromiter(map(len, rows), dtype=np.int64, count=len(rows))
+    flat = np.array([r[:3] for row in rows for r in row], dtype=np.float32).reshape(-1, 3)
+    n, width = len(rows), max(1, int(lens.max(initial=0)))
+    valid = np.arange(width)[None, :] < lens[:, None]
+    packed = np.zeros((n, width, 3), dtype=np.float32)
+    packed[valid] = flat
+    return packed[..., 0], packed[..., 1], packed[..., 2], valid
+
+
+def _pack_ground_truth(items, video2idx, need_ts, use_desc_type):
+    """GT dicts -> clip index (n,), spans float32 (n, T, 2) with their mask (n, T), the DiDeMo
+    flag (n,) (>= 4 spans: a hit needs 2 overlaps) and the desc type index (n,)."""
+    n = len(items)
+    gvid = np.array([video2idx[e["vid_name"]] for e in items], dtype=np.int64)
+    dtype = np.zeros(n, dtype=np.int64)
+    if use_desc_type:
+        bad = {e.get("type") for e in items} - set(DESC_TYPES)
+        if bad:
+            raise ValueError(f"desc types {sorted(map(str, bad))}: expected one of {DESC_TYPES}")
+        dtype = np.array([DESC_TYPES.index(e["type"]) for e in items], dtype=np.int64)
+    if not need_ts:
+        return gvid, None, None, None, dtype
+    spans = []
+    for e in items:
+        if "ts" not in e:
+            raise ValueError(f"ground truth of desc_id {e['desc_id']} has no 'ts'")
+        ts = np.asarray(e["ts"], dtype=np.float32)
+        if ts.shape == (2,):
+            ts = ts[None]
+        elif not (ts.ndim == 2 and ts.shape[1] == 2 and len(ts) >= 4):
+            raise ValueError(f"ground truth 'ts' of desc_id {e['desc_id']} with shape {ts.shape}: "
+                             "expected [st, ed] or at least 4 [st, ed] pairs")
+        spans.append(ts)
+    width = max(len(s) for s in spans) if spans else 1
+    gts = np.zeros((n, width, 2), dtype=np.float32)
+    on = np.zeros((n, width), dtype=bool)
+    for i, s in enumerate(spans):
+        gts[i, :len(s)] = s
+        on[i, :len(s)] = True
+    return gvid, gts, on, on.sum(1) >= 4, dtype
+
+
+def _task_metrics(task, vid, st, ed, valid, gt, iou_thds, use_desc_type):
+    """eval_by_task_type (utils/tvr_standalone_eval.py:86-257) on packed predictions, vectorised
+    over queries: float32 predictions and IoU, `>=` each threshold, the same float64 means."""
+    gvid, gts, on, didemo, dtype = gt
+    matched = valid & (vid == gvid.astype(np.float32)[:, None])       # (n, P)
+    metrics, by_type = OrderedDict(), OrderedDict()
+    n_type = [np.sum(dtype == t) for t in range(len(DESC_TYPES))]
+
+    def put(key_fmt, hit_of_k, *key_args):
+        for k in RECALL_TOPKS:
+            metrics[key_fmt.format(*key_args, k)] = _rounded_percentage(np.mean(hit_of_k(k)))
+        return hit_of_k
+
+    hits = []                                   # (key prefix, hit_of_k)
+    if task == "VR":
+        hits.append(("", put("r{}", lambda k: matched[:, :k].any(1))))
+    else:
+        inter = np.maximum(0, np.minimum(ed[:, :, None], gts[:, None, :, 1])
+                           - np.maximum(st[:, :, None], gts[:, None, :, 0]))
+        union = np.maximum(ed[:, :, None], gts[:, None, :, 1]) - np.minimum(st[:, :, None],
+                                                                            gts[:, None, :, 0])
+        iou = np.divide(inter, union, out=np.zeros_like(inter), where=union != 0)
+        iou = iou * matched[:, :, None]         # wrong clip: IoU 0
+        rank_in_clip = np.cumsum(matched, axis=1)
+        for thd in iou_thds:
+            ok = (iou >= thd) & on[:, None, :] & valid[:, :, None]             # (n, P, T)
+            corr = np.where(didemo[:, None], ok.sum(-1) >= 2, ok[:, :, 0])
+            if task == "VCMR":
+                fn = (lambda c: lambda k: c[:, :k].any(1))(corr)
+            else:                               # SVMR: the first k clip-matched predictions
+                fn = (lambda c: lambda k: (c & matched & (rank_in_clip <= k)).any(1))(corr)
+            hits.append((f"{thd}-", put("{}-r{}", fn, thd)))
+    if use_desc_type:
+        with np.errstate(invalid="ignore", divide="ignore"):
+            for t, name in enumerate(DESC_TYPES):
+                is_t = dtype == t
+                for prefix, fn in hits:
+                    for k in RECALL_TOPKS:
+                        by_type[f"{name}-{prefix}r{k}"] = _rounded_percentage(
+                            1.0 * np.sum(np.logical_and(fn(k), is_t)) / n_type[t])
+            by_type["desc_type_ratio"] = "v {} t {} vt {}".format(
+                *[_rounded_percentage(1.0 * n_type[t] / len(dtype)) for t in range(3)])
+    return metrics, by_type
+
+
+def _metrics(packed_by_task, ground_truth, video2idx, iou_thds, use_desc_type, match_number):
+    """eval_retrieval on {task: (desc_ids, vid, st, ed, valid)}."""
+    gt_by_id = {e["desc_id"]: e for e in ground_truth}
+    out, by_type = OrderedDict(), OrderedDict()
+    for task in TVR_TASKS:
+        if task not in packed_by_task:
+            continue
+        desc_ids, vid, st, ed, valid = packed_by_task[task]
+        pos = {d: i for i, d in enumerate(desc_ids)}
+        if match_number and set(gt_by_id) != set(pos):
+            raise ValueError(f"{task}: desc_ids in predictions and ground_truth must match")
+        keys = [k for k in gt_by_id if k in pos]
+        rows = np.array([pos[k] for k in keys], dtype=np.int64)
+        gt = _pack_ground_truth([gt_by_id[k] for k in keys], video2idx, task != "VR",
+                                use_desc_type)
+        out[task], by_type[task + "_by_type"] = _task_metrics(
+            task, vid[rows], st[rows], ed[rows], valid[rows], gt, iou_thds, use_desc_type)
+    if use_desc_type:
+        out.update(by_type)
+    return out
+
+
+def eval_retrieval(submission, ground_truth, iou_thds=(0.5, 0.7), use_desc_type=True,
+                   match_number=True):
+    """The reference's `eval_retrieval` (utils/tvr_standalone_eval.py:260-283) for a submission
+    ({"VCMR", "SVMR", "VR"} lists of dict(desc_id, predictions) and "video2idx") against
+    ground-truth dicts (desc_id, vid_name, ts, type): R@{1,5,10,100} at each IoU threshold over
+    the first 100 predictions, equal (not just close) to the reference's OrderedDicts, with
+    "<task>_by_type" entries when use_desc_type.
+
+    Precision follows the reference: predictions (clip index included) in float32, IoU in float32
+    and 0 for a prediction of the wrong clip, `>=` the threshold; SVMR counts only clip-matched
+    predictions; ground truth with at least 4 `ts` pairs (DiDeMo) counts a hit when 2 or more
+    overlap. Raises ValueError for `ts` of 2 or 3 pairs, unknown desc types and, under
+    match_number, desc_id sets that differ between a task's predictions and the ground truth."""
+    packed = {}
+    for task in TVR_TASKS:
+        if task in submission:
+            by_id = {e["desc_id"]: e for e in submission[task]}
+            ids = list(by_id)
+            packed[task] = (ids, *_pack_lists([by_id[d]["predictions"] for d in ids]))
+    return _metrics(packed, ground_truth, submission["video2idx"], iou_thds, use_desc_type,
+                    match_number)
+
+
+def _packed_moments(score, mom, lookup, interval, svmr):
+    """Host arrays of one task -> (vid int64, st, ed, score, valid), times as _moment_records."""
+    valid = mom[..., 0] >= 0
+    vid = np.where(valid, lookup[np.maximum(mom[..., 0], 0)], 0)
+    if svmr:
+        st = mom[..., 1].astype(np.float64) * interval
+        ed = (mom[..., 2].astype(np.float64) + 1) * interval
+    else:
+        st = mom[..., 1].astype(np.float32) * interval
+        ed = mom[..., 2].astype(np.float32) * interval + interval
+    return vid, st, ed, score, valid
+
+
+def _records(qids, vid, st, ed, score, valid):
+    n = valid.sum(1).tolist()
+    vid, st, ed, score = vid.tolist(), st.tolist(), ed.tolist(), score.tolist()
+    return [dict(desc_id=int(q), desc="", predictions=[
+        list(r) for r in zip(vid[i][:c], st[i][:c], ed[i][:c], score[i][:c])])
+        for i, (q, c) in enumerate(zip(qids, n))]
+
+
+def full_vcmr_eval(model, corpus, batches, video_ids, video2idx, ground_truth, *,
+                   tasks=RANK_TASKS, q2c_alpha=20.0, max_vcmr_video=100, min_pred_l=2,
+                   max_pred_l=16, max_before_nms=200, max_after_nms=100, nms_thd=0.5,
+                   vfeat_interval=1.5, use_desc_type=True):
+    """The reference's full VCMR evaluation from ranking to metrics (validate_full_vcmr,
+    eval_vcmr.py:205-508, one process): rank every query batch, run NMS on the device, copy both
+    lists to the host in the batch's one copy, and score them with `eval_retrieval`'s arithmetic
+    on the packed arrays.
+
+    Arguments as `full_vcmr_predictions`, plus ground_truth: the GT dicts of the evaluated queries
+    (the reference's partial_query_data), or None. Returns {"submission": the top-max_after_nms
+    lists as get_submission_top_n leaves them, "metrics": eval_retrieval of those}; with
+    nms_thd != -1 also {"submission_nms": {"video2idx", "SVMR", "VCMR"} after NMS, "metrics_nms"}.
+    Metrics are given only when every batch has targets and ground_truth is not None.
+
+    This reproduces what the reference effectively does:
+    * get_submission_top_n (eval_vcmr.py:420) truncates the eval_res lists in place, so its NMS
+      reads only the first min(max_before_nms, max_after_nms) predictions, not max_before_nms.
+    * The same aliasing makes the reference return the post-NMS SVMR / VCMR lists as its
+      eval_submission; both are returned here, explicitly.
+    * NMS keeps at most 100 moments per clip (the inner default of temporal_non_maximum_suppression)
+      whatever max_after_nms is.
+    Deviations: those of `full_vcmr_predictions`, and an SVMR query without any band-valid span
+    gets an empty list where the reference raises IndexError (tvr_eval_utils.py:231). The
+    reference computes the post-NMS lists only when it has ground truth."""
+    tasks = _vcmr_tasks(model, tasks)
+    if max_after_nms < 1:
+        raise ValueError(f"max_after_nms = {max_after_nms} < 1")
+    do_nms = nms_thd != -1
+    n_top = min(max_before_nms, max_after_nms)
+    n_vr = min(100, max_after_nms)
+
+    def post(out):
+        res = {}
+        if "VR" in out:
+            res["VR"] = tuple(t[:, :n_vr] for t in out["VR"])
+        for t in ("VCMR", "SVMR"):
+            if t in out:
+                s, m = out[t]
+                res[t] = (s[:, :n_top], m[:, :n_top])
+                if do_nms:
+                    res[t + "_NMS"] = nms_moments(s, m, nms_thd=nms_thd, n_in=n_top, n_out=n_top,
+                                                  interval=vfeat_interval, by_clip=t == "VCMR")
+        return res
+
+    qids, results, has_gt = [], [], False
+    if tasks:
+        rank_kw = dict(tasks=tasks, q2c_alpha=q2c_alpha, max_video=max_vcmr_video,
+                       min_pred_l=min_pred_l, max_pred_l=max_pred_l, max_before_nms=max_before_nms)
+        qids, results, has_gt = _run_batches(model, corpus, batches, video_ids, rank_kw, True,
+                                             post)
+    lookup = np.array([video2idx[v] for v in video_ids], dtype=np.int64)
+
+    def task_arrays(key, svmr):
+        parts = [r[key] for r in results if key in r]
+        if not parts or (svmr and not has_gt):
+            return None
+        score, mom = (np.concatenate(x) for x in zip(*parts))
+        if key == "VR":
+            vid = lookup[mom]
+            zeros = np.zeros(vid.shape, dtype=np.int64)
+            return vid, zeros, zeros, score, np.ones(vid.shape, dtype=bool)
+        return _packed_moments(score, mom, lookup, vfeat_interval, svmr)
+
+    def build(keys):
+        sub, packed = {}, {}
+        for task, key in keys:
+            arr = task_arrays(key, task == "SVMR")
+            if arr is None or not qids:
+                continue
+            vid, st, ed, score, valid = arr
+            sub[task] = _records(qids, *arr)
+            packed[task] = ([int(q) for q in qids], vid.astype(np.float32),
+                            np.asarray(st, dtype=np.float32), np.asarray(ed, dtype=np.float32),
+                            valid)
+        sub = {k: sub[k] for k in ("SVMR", "VCMR", "VR") if k in sub}
+        sub["video2idx"] = video2idx
+        return sub, packed
+
+    with_metrics = has_gt and ground_truth is not None
+    iou_thds = (0.5, 0.7)                      # VCMR_IOU_THDS (utils/const.py)
+    out = {}
+    out["submission"], packed = build([("SVMR", "SVMR"), ("VCMR", "VCMR"), ("VR", "VR")])
+    if with_metrics:
+        out["metrics"] = _metrics(packed, ground_truth, video2idx, iou_thds, use_desc_type, True)
+    if do_nms:
+        out["submission_nms"], packed = build([("SVMR", "SVMR_NMS"), ("VCMR", "VCMR_NMS")])
+        if with_metrics:
+            out["metrics_nms"] = _metrics(packed, ground_truth, video2idx, iou_thds,
+                                          use_desc_type, True)
+    return out
 
 
 class ModelSaver(object):

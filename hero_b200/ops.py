@@ -581,6 +581,22 @@ def vcmr_moment_topn(st, ed, video_factor, nq, k, length, min_l, max_l, n, score
                                                 _stream()))
 
 
+def temporal_nms(score, mom, n_in, thd, interval, by_clip, n_out, out_score, out_mom):
+    """out_score [nq, n_out] / out_mom [nq, n_out, 3] = greedy temporal NMS (IoU > thd suppressed,
+    at most 100 kept per group) of the first n_in entries of each ranked row of score [nq, ld] /
+    mom [nq, ld, 3]; by_clip groups by clip row (VCMR), otherwise one group (SVMR)."""
+    _require_cuda(score, mom, out_score, out_mom)
+    assert score.dtype == torch.float32 and out_score.dtype == torch.float32
+    assert mom.dtype == torch.int32 and out_mom.dtype == torch.int32
+    assert score.stride(1) == 1 and mom.stride(2) == 1 and mom.stride(1) == 3
+    assert mom.stride(0) == 3 * score.stride(0)
+    assert out_score.is_contiguous() and out_mom.is_contiguous()
+    _count()
+    _lib.check(_lib.lib().hero_temporal_nms(_ptr(score), _ptr(mom), score.shape[0], score.stride(0),
+                                            n_in, float(thd), float(interval), int(by_clip), n_out,
+                                            _ptr(out_score), _ptr(out_mom), _stream()))
+
+
 # ---------------------------------------------------------------------------------------------
 # Fused LM-head cross entropy (MLM): vocabulary logits are never materialised in fp32.
 def lm_head_ce_fwd(h, emb, bias, labels, n_valid):

@@ -484,6 +484,23 @@ int hero_vcmr_moment_topn(const float* st, const float* ed, const float* video_f
                           int32_t k, int32_t len, int32_t min_l, int32_t max_l, int32_t n,
                           float* score, int32_t* jse, void* stream);
 
+/* ---- temporal NMS of ranked moment lists (hero_b200/csrc/nms.cu) ----
+ * Replaces the reference's host post-processing: temporal_non_maximum_suppression,
+ * filter_vcmr_by_nms, post_processing_vcmr_nms / post_processing_svmr_nms
+ * (utils/tvr_eval_utils.py:35-92, 132-234). Per query q (one CTA), reads the first n_in <= 1024
+ * entries of score [nq, ld_in] and mom [nq, ld_in, 3] = (clip row, s, e), sorted by descending
+ * score, up to the first entry with mom < 0. Times: by_clip (VCMR) st = f32(s)*f32(iv), ed =
+ * f32(e)*f32(iv) + f32(iv), each step rounded in fp32; otherwise (SVMR) st = s*iv, ed = (e+1)*iv in
+ * fp64. IoU = max(0, min(ed) - max(st)) / (max(ed) - min(st)) in fp64 (0 when the hull is empty).
+ * Greedy NMS in score order within each group (by_clip: one group per clip row; otherwise one group):
+ * keep the best alive entry, drop the later ones of its group with IoU > thd, at most 100 kept per
+ * group. The kept entries are stable-sorted by descending score over the groups concatenated in
+ * order of first appearance, and the first n_out <= 1024 are written to out_score [nq, n_out] and
+ * out_mom [nq, n_out, 3]; the tail is score 0, mom -1. */
+int hero_temporal_nms(const float* score, const int32_t* mom, int32_t nq, int32_t ld_in,
+                      int32_t n_in, double thd, double interval, int32_t by_clip, int32_t n_out,
+                      float* out_score, int32_t* out_mom, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
