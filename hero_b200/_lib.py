@@ -152,6 +152,11 @@ def _declare(lib):
         vp)
     sig("hero_vcmr_moment_topn", vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp)
     sig("hero_temporal_nms", vp, vp, i32, i32, i32, C.c_double, C.c_double, i32, i32, vp, vp, vp)
+    sig("hero_qa_pool_fwd", vp, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp)
+    lib.hero_qa_pool_bwd_scratch_floats.restype = C.c_int64
+    lib.hero_qa_pool_bwd_scratch_floats.argtypes = [i32, i32, i32, i32]
+    sig("hero_qa_pool_bwd", vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp,
+        vp)
 
 
 def lib():

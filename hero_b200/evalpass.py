@@ -15,6 +15,7 @@
   temporal NMS of the ranked lists on the device (csrc/nms.cu), carried home in the same copy, and
   the TVR recall metrics of utils/tvr_standalone_eval.py vectorised over queries on the host
   (DESIGN §4 "Temporal NMS and TVR metrics").
+* `validate_videoqa` — eval_videoQA.py:120-173 for one process on HeroForVideoQA.
 * `ModelSaver` / `TrainingRestorer` — utils/save.py:112-181 with the same file layout (`vocab_padded`
   flag, `model_step_<n>.pt`, `train_state_<n>.pt`, `restore.pt` + backup), so checkpoints are
   interchangeable with the reference's; optimizer state is FusedAdamW's flat moments.
@@ -728,6 +729,55 @@ def full_vcmr_eval(model, corpus, batches, video_ids, video2idx, ground_truth, *
             out["metrics_nms"] = _metrics(packed, ground_truth, video2idx, iou_thds,
                                           use_desc_type, True)
     return out
+
+
+@torch.no_grad()
+def validate_videoqa(model, loader, split, task="tvqa", save_logits=False):
+    """eval_videoQA.py:120-173 (validate_videoQA) for one process: returns (val_log, results,
+    logits) with `valid/loss`, `valid/acc`, `valid/ex_per_s`, results[str(qid)] = predicted answer
+    index and, with `save_logits`, logits[str(qid)] = the candidate logits. Once a batch carries a
+    negative target ("no ground truth") only predictions are made and val_log stays empty, as in
+    the reference. Loss sums and correct counts are computed on the device; each batch makes one
+    device->host copy (answers, loss sum, correct count, smallest target, logits). Averaging across
+    ranks (all_gather_list) is left to the caller. `split` names the split only."""
+    import time
+    model.eval()
+    val_loss, n_ex, tot_score = 0.0, 0, 0
+    results, logits, val_log = {}, {}, {}
+    t0 = time.time()
+    has_gt_target = True
+    for batch in loader:
+        qids = batch.pop("qids")
+        targets = batch["targets"]
+        scores = model(batch, task, compute_loss=False)                 # (Nv, Nq)
+        tgt = targets.to(scores.device).reshape(-1)
+        answers = scores.max(dim=-1)[1]
+        loss = torch.nn.functional.cross_entropy(scores, tgt.clamp(min=0), reduction="sum")
+        correct = (answers == tgt).sum()
+        packed = torch.cat([answers.float(), loss.reshape(1).float(), correct.reshape(1).float(),
+                            tgt.min().reshape(1).float()] +
+                           ([scores.float().reshape(-1)] if save_logits else []))
+        host = packed.cpu()
+        n = answers.numel()
+        ans = host[:n].long().tolist()
+        b_loss, b_correct, b_min = (float(x) for x in host[n:n + 3])
+        if has_gt_target and b_min < 0:
+            has_gt_target = False
+        for qid, answer in zip(qids, ans):
+            results[str(qid)] = answer
+        if save_logits:
+            for qid, row in zip(qids, host[n + 3:].view(n, -1).tolist()):
+                logits[str(qid)] = row
+        if has_gt_target:
+            val_loss += b_loss
+            tot_score += int(b_correct)
+            n_ex += len(qids)
+    if has_gt_target:
+        tot_time = time.time() - t0
+        val_log = {"valid/loss": val_loss / n_ex, "valid/acc": tot_score / n_ex,
+                   "valid/ex_per_s": n_ex / tot_time}
+    model.train()
+    return val_log, results, logits
 
 
 class ModelSaver(object):

@@ -9,6 +9,8 @@ gradients; the arithmetic reads the bf16 working copies held in `ctx_w` objects.
     cross_modal_embed   _compute_img_txt_embeddings   model/encoder.py:256-285 (+ embed.py:28-117)
     frame_merge         collect_frame_outputs + frame_transform residual  model/model.py:156-212
     frame_embed         FrameEmbeddings               model/embed.py:146-161
+    qa_fused_embed      frame + question/answer embeddings of video QA  model/videoQA.py:68-78
+    qa_pool             both attention poolings of video QA             model/videoQA.py:36-59
     pack / unpack       padded <-> packed layouts
 """
 import torch
@@ -459,6 +461,124 @@ class _FrameEmbed(torch.autograd.Function):
 
 def frame_embed(g, cfg, params):
     return _FrameEmbed.apply(g, cfg, *params)
+
+
+class _QaFusedEmbed(torch.autograd.Function):
+    """Query-fused embeddings of video QA (model/videoQA.py:68-78) written into ONE packed buffer
+    at the rows of plan.QaPlan, by two launches of the existing gather + add + LayerNorm kernel
+    (its destination-row map `y_rows` places each half):
+        frame token k:  LN_c(g[k] + c_pos[t_k])                    c_encoder.embeddings
+        QA token:       LN_f(word[id] + f_pos[p] + type[1])        f_encoder.embeddings
+    each followed by dropout with its own module's probability (cfg "frm_p" / "qa_p", 0 in eval).
+    params: c_pos, c_ln_w, c_ln_b, word, f_pos, type, f_ln_w, f_ln_b.
+    Returns (bf16 operand, fp32 residual copy) like cross_modal_embed / frame_embed."""
+
+    @staticmethod
+    def forward(ctx, g, cfg, *params):
+        c_pos, c_ln_w, c_ln_b, word, f_pos, typ, f_ln_w, f_ln_b = params
+        drop, dev = cfg["drop"], g.device
+        n_tok, n_frm, n_qa = cfg["n_tok"], cfg["n_frm"], cfg["n_qa"]
+        H = g.shape[1]
+        emb = torch.empty((n_tok, H), dtype=BF16, device=dev)
+        emb32 = torch.empty((n_tok, H), dtype=F32, device=dev)
+        st = {"f_mean": torch.empty(n_frm, device=dev), "f_rstd": torch.empty(n_frm, device=dev),
+              "q_mean": torch.empty(n_qa, device=dev), "q_rstd": torch.empty(n_qa, device=dev),
+              "f_drop": drop.next(cfg["frm_p"]), "q_drop": drop.next(cfg["qa_p"])}
+        if n_frm:
+            ops.ln_fwd(g, c_ln_w, c_ln_b, 1e-5, emb, n_rows=n_frm, add_tab=c_pos,
+                       add_idx=cfg["frm_t"], y_rows=cfg["frm_tok"], mean=st["f_mean"],
+                       rstd=st["f_rstd"], drop=st["f_drop"], y_f32=emb32)
+        if n_qa:
+            ops.ln_fwd(word, f_ln_w, f_ln_b, 1e-5, emb, n_rows=n_qa, x_rows=cfg["qa_ids"],
+                       add_tab=f_pos, add_idx=cfg["qa_pos"], add_vec=typ[1],
+                       y_rows=cfg["qa_tok"], mean=st["q_mean"], rstd=st["q_rstd"],
+                       drop=st["q_drop"], y_f32=emb32)
+        ctx.cfg, ctx.st, ctx.params = cfg, st, params
+        ctx.save_for_backward(g)
+        ctx.mark_non_differentiable(emb32)
+        return emb, emb32
+
+    @staticmethod
+    def backward(ctx, demb, _demb32=None):
+        cfg, st = ctx.cfg, ctx.st
+        c_pos, c_ln_w, c_ln_b, word, f_pos, typ, f_ln_w, f_ln_b = ctx.params
+        (g,) = ctx.saved_tensors
+        demb = demb.contiguous()
+        n_frm, n_qa = cfg["n_frm"], cfg["n_qa"]
+        H = g.shape[1]
+        grads = [None] * 8
+        dg = torch.empty((n_frm, H), dtype=BF16, device=g.device)
+        if n_frm:
+            dlnw, grads[1] = _sink(c_ln_w)
+            dlnb, grads[2] = _sink(c_ln_b)
+            ops.ln_bwd(demb, g, c_ln_w, st["f_mean"], st["f_rstd"], n_rows=n_frm, add_tab=c_pos,
+                       add_idx=cfg["frm_t"], y_rows=cfg["frm_tok"], drop=st["f_drop"], dx=dg,
+                       dgamma=dlnw, dbeta=dlnb)
+            dpos, grads[0] = _sink(c_pos)
+            n_slot = cfg["cpos_off"].numel() - 1
+            ops.gather_sum_rows(dg, cfg["cpos_off"], cfg["cpos_idx"], dpos[:n_slot])
+        if n_qa:
+            dword, grads[3] = _sink(word)
+            dlnw, grads[6] = _sink(f_ln_w)
+            dlnb, grads[7] = _sink(f_ln_b)
+            dx = torch.empty((n_qa, H), dtype=BF16, device=g.device)
+            ops.ln_bwd(demb, word, f_ln_w, st["q_mean"], st["q_rstd"], n_rows=n_qa,
+                       x_rows=cfg["qa_ids"], add_tab=f_pos, add_idx=cfg["qa_pos"], add_vec=typ[1],
+                       y_rows=cfg["qa_tok"], drop=st["q_drop"], dx=dx, d_x_tab=dword,
+                       x_pad_idx=cfg["pad_idx"], dgamma=dlnw, dbeta=dlnb)
+            dpos, grads[4] = _sink(f_pos)
+            n_slot = cfg["qpos_off"].numel() - 1
+            ops.gather_sum_rows(dx, cfg["qpos_off"], cfg["qpos_idx"], dpos[:n_slot])
+            dtyp, grads[5] = _sink(typ)
+            ops.colsum(dx, dtyp[1])
+        ctx.st = None
+        return (dg, None) + tuple(grads)
+
+
+def qa_fused_embed(g, cfg, params):
+    return _QaFusedEmbed.apply(g, cfg, *params)
+
+
+class _QaPool(torch.autograd.Function):
+    """Both attention poolings of video QA (model/videoQA.py:36-59) on the packed fp32 temporal
+    outputs h: qa_pooled (Nv*Nq, H) over the frames of each candidate, st_pooled (Nv*L, H) over
+    the candidates of each frame (csrc/qa.cu)."""
+
+    @staticmethod
+    def forward(ctx, h, w_qa, w_st, frame_map, mask, dims):
+        nv, nq, length = dims
+        H = h.shape[1]
+        h = h.contiguous()
+        wq = w_qa.detach().float().reshape(-1).contiguous()
+        ws = w_st.detach().float().reshape(-1).contiguous()
+        mask = mask.float().reshape(-1).contiguous()
+        a = torch.empty(nv * nq * length, dtype=F32, device=h.device)
+        b = torch.empty_like(a)
+        qa = torch.empty((nv * nq, H), dtype=F32, device=h.device)
+        sp = torch.empty((nv * length, H), dtype=F32, device=h.device)
+        ops.qa_pool_fwd(h, frame_map, mask, wq, ws, nv, nq, length, a, b, qa, sp)
+        ctx.st = (h, wq, ws, frame_map, mask, a, b, dims)
+        ctx.w_shape = tuple(w_qa.shape)
+        return qa, sp
+
+    @staticmethod
+    def backward(ctx, d_qa, d_st):
+        h, wq, ws, frame_map, mask, a, b, (nv, nq, length) = ctx.st
+        dh = torch.zeros_like(h)                 # question / answer rows get no gradient here
+        dwq, dws = torch.zeros_like(wq), torch.zeros_like(ws)
+        z = lambda t, shape: torch.zeros(shape, dtype=F32, device=h.device) if t is None \
+            else t.float().contiguous()
+        ops.qa_pool_bwd(h, frame_map, mask, wq, ws, a, b, z(d_qa, (nv * nq, h.shape[1])),
+                        z(d_st, (nv * length, h.shape[1])), nv, nq, length, dh, dwq, dws)
+        ctx.st = None
+        return dh, dwq.view(ctx.w_shape), dws.view(ctx.w_shape), None, None, None
+
+
+def qa_pool(h, w_qa, w_st, frame_map, mask, nv, nq, length):
+    """h fp32 [n_tok, H]; frame_map int32 [Nv*Nq*L] (plan.QaPlan); mask [Nv*Nq*L] 0/1.
+    Bounds (ValueError before any launch): Nq <= 16, L <= 512, H a multiple of 8."""
+    ops._qa_bounds(nv, nq, length, h.shape[1])
+    return _QaPool.apply(h, w_qa, w_st, frame_map, mask, (nv, nq, length))
 
 
 # ---------------------------------------------------------------------------------------------

@@ -16,7 +16,7 @@ import collections
 
 import torch
 
-from .plan import PLAN_KEY, PlanPool, attach_plan
+from .plan import PLAN_KEY, QA_PLAN_KEY, PlanPool, attach_plan, video_kind
 
 
 class BatchStager:
@@ -68,6 +68,10 @@ class BatchStager:
                     if joint is not None:
                         joint.dev = None
                         joint.to(self.device, self._staging(bufs, (bi, "joint")))
+                qplan = d.get(QA_PLAN_KEY)
+                if qplan is not None:     # video QA: the query-fused rows' plan likewise
+                    qplan.dev = None
+                    qplan.to(self.device, self._staging(bufs, (bi, "qa")))
                 out.append(d)
             ready = torch.cuda.Event()
             ready.record(self.stream)
@@ -99,14 +103,15 @@ def record_plans(batches, stream):
         plan = b.get(PLAN_KEY)
         if plan is None:
             continue
-        for p in (plan, plan.__dict__.get("_joint")):
+        for p in (plan, plan.__dict__.get("_joint"), b.get(QA_PLAN_KEY)):
             if p is not None and p.dev is not None:
                 p.dev.flat.record_stream(stream)
 
 
 class PrefetchLoader:
     """data/loader.py:89-144 on a BatchStager. `loader` yields host batches: a dict (video batch,
-    'repr' plan) or a (video_dict, query_dict) pair for the fused `forward_repr_txt` path. Plans
+    'repr' plan; a video_qa_collate batch gets the 'videoqa' plans) or a (video_dict, query_dict)
+    pair for the fused `forward_repr_txt` path. Plans
     already attached by the collate function are used as they are; otherwise they are built two
     batches ahead in `plan_workers` processes (0: in this process)."""
 
@@ -144,7 +149,7 @@ class PrefetchLoader:
             if fut is not None:
                 PlanPool.attach(fut, vb, qb)
             elif need:
-                attach_plan(vb)
+                attach_plan(vb, kind=video_kind(vb))
                 if qb is not None:
                     attach_plan(qb, kind="txt")
             yield (vb, qb) if pair else vb

@@ -646,3 +646,48 @@ def lm_head_ce_dlogits(h, emb, bias, labels, lse, grad, n_valid, out):
     _count()
     _lib.check(_lib.lib().hero_gemm_bf16(C.byref(g), _stream()))
     return out
+
+
+# ---------------------------------------------------------------------------------------------
+# Video QA attention pooling (hero_b200/csrc/qa.cu)
+QA_MAX_NQ, QA_MAX_L = 16, 512
+
+
+def _qa_bounds(nv, nq, length, h):
+    if nv < 1 or not 1 <= nq <= QA_MAX_NQ or not 1 <= length <= QA_MAX_L or h < 8 or h % 8:
+        raise ValueError(f"qa_pool: (Nv, Nq, L, H) = ({nv}, {nq}, {length}, {h}); the kernels take "
+                         f"Nv >= 1, 1 <= Nq <= {QA_MAX_NQ}, 1 <= L <= {QA_MAX_L} and H a positive "
+                         f"multiple of 8")
+
+
+def qa_pool_fwd(h, frame_map, mask, w_qa, w_st, nv, nq, length, a, b, qa_pooled, st_pooled):
+    """Both attention poolings of model/videoQA.py:36-59 over the packed fp32 rows h [*, H]:
+    a / b [Nv*Nq*L] pooling weights, qa_pooled [Nv*Nq, H], st_pooled [Nv*L, H] (`hero_qa_pool_fwd`)."""
+    _require_cuda(h, frame_map, mask, w_qa, w_st, a, b, qa_pooled, st_pooled)
+    H = h.shape[1]
+    _qa_bounds(nv, nq, length, H)
+    for t in (h, mask, w_qa, w_st, a, b, qa_pooled, st_pooled):
+        assert t.dtype == torch.float32 and t.is_contiguous()
+    assert frame_map.dtype == torch.int32 and frame_map.numel() == nv * nq * length
+    _count(2)
+    _lib.check(_lib.lib().hero_qa_pool_fwd(_ptr(h), _ptr(frame_map), _ptr(mask), _ptr(w_qa),
+                                           _ptr(w_st), nv, nq, length, H, _ptr(a), _ptr(b),
+                                           _ptr(qa_pooled), _ptr(st_pooled), _stream()))
+
+
+def qa_pool_bwd(h, frame_map, mask, w_qa, w_st, a, b, d_qa, d_st, nv, nq, length, dh, dw_qa,
+                dw_st):
+    """Backward of qa_pool_fwd (`hero_qa_pool_bwd`): writes the frame rows of dh, accumulates
+    dw_qa / dw_st (fp32 [H]) in a fixed order."""
+    _require_cuda(h, frame_map, mask, w_qa, w_st, a, b, d_qa, d_st, dh, dw_qa, dw_st)
+    H = h.shape[1]
+    _qa_bounds(nv, nq, length, H)
+    for t in (h, mask, w_qa, w_st, a, b, d_qa, d_st, dh, dw_qa, dw_st):
+        assert t.dtype == torch.float32 and t.is_contiguous()
+    n = _lib.lib().hero_qa_pool_bwd_scratch_floats(nv, nq, length, H)
+    scratch = torch.empty(n, dtype=torch.float32, device=h.device)
+    _count(4)
+    _lib.check(_lib.lib().hero_qa_pool_bwd(_ptr(h), _ptr(frame_map), _ptr(mask), _ptr(w_qa),
+                                           _ptr(w_st), _ptr(a), _ptr(b), _ptr(d_qa), _ptr(d_st),
+                                           nv, nq, length, H, _ptr(scratch), _ptr(dh),
+                                           _ptr(dw_qa), _ptr(dw_st), _stream()))

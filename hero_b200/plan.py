@@ -414,7 +414,67 @@ class JointPlan:
                 "n_tok": self.n_tok, "n_seq": self.n_seq, "max_len": self.max_len}
 
 
+class QaPlan:
+    """Query-fused temporal rows of video QA (model/videoQA.py:68-86): row r = (video v, candidate
+    q) of the collate (video-major, Nq = rows / Nv) is [valid frames of c_attn_masks[r] | valid
+    tokens of qa_attn_masks[r]], each sequence contiguous in one packed buffer. Frames keep their
+    column as temporal position; question / answer tokens take `qa_pos_ids`.
+
+    Frame tokens appear in the same row-major order as CPlan's clip tokens, so frame k of the
+    packed stream reads row k of the cross-modal output `g` (no source map needed)."""
+
+    def __init__(self, c_attn_masks, qa_attn_masks, qa_input_ids, qa_pos_ids, n_videos):
+        cm, qm = _np(c_attn_masks) != 0, _np(qa_attn_masks) != 0
+        rows, L = cm.shape
+        if qm.shape[0] != rows:
+            raise ValueError(f"qa_attn_masks has {qm.shape[0]} rows, c_attn_masks {rows}")
+        if n_videos < 1 or rows % n_videos:
+            raise ValueError(f"{rows} query-fused rows do not split into {n_videos} videos")
+        self.n_videos, self.n_cand, self.length = int(n_videos), rows // int(n_videos), L
+        # attention tiles of the joint rows; a row over ATTN_LONG_MAX tokens raises here
+        self.seq = SeqPlan(np.concatenate([cm, qm], 1))
+        s = self.seq
+        tok = np.arange(s.n_tok, dtype=np.int32)
+        is_frm = s.tok_col < L
+        self.frm_tok = tok[is_frm]                                    # packed row of frame k
+        self.frm_t = s.tok_col[is_frm].astype(np.int32)               # its temporal position
+        self.qa_tok = tok[~is_frm]
+        qa_row, qa_j = s.tok_row[~is_frm], (s.tok_col[~is_frm] - L).astype(np.int64)
+        ids = np.asarray(_np(qa_input_ids), np.int64)
+        pos = np.asarray(_np(qa_pos_ids), np.int64)
+        pos = pos.reshape(1, -1) if pos.ndim == 1 else pos
+        self.qa_ids = ids[qa_row, qa_j].astype(np.int32)
+        self.qa_pos = (pos[0][qa_j] if pos.shape[0] == 1 else pos[qa_row, qa_j]).astype(np.int32)
+        self.n_frm, self.n_qa = int(self.frm_tok.size), int(self.qa_tok.size)
+        # deterministic position-table gradients: CSR over the position ids actually used
+        self.cpos_off, self.cpos_idx = table_csr(self.frm_t, max(L, 1))
+        n_qpos = int(self.qa_pos.max()) + 1 if self.n_qa else 1
+        self.qpos_off, self.qpos_idx = table_csr(self.qa_pos, n_qpos)
+        # (v, q, l) -> packed row of that frame, -1 for padding (read by the pooling kernels)
+        fmap = np.full(rows * L, -1, np.int32)
+        fmap[s.tok_row[is_frm].astype(np.int64) * L + self.frm_t] = self.frm_tok
+        self.frame_map = fmap
+        self.n_long_rows = int(s.n_long)
+        self.dev = None
+
+    def to(self, device, staging=None):
+        device = torch.device(device)
+        if self.dev is None or self.dev.flat.device != device:
+            a = {"cu": self.seq.cu, "seq_lo": self.seq.seq_lo, "seq_hi": self.seq.seq_hi,
+                 "tile_tok0": self.seq.tile_tok0, "tile_ntok": self.seq.tile_ntok,
+                 "frm_tok": self.frm_tok, "frm_t": self.frm_t, "qa_tok": self.qa_tok,
+                 "qa_ids": self.qa_ids, "qa_pos": self.qa_pos, "cpos_off": self.cpos_off,
+                 "cpos_idx": self.cpos_idx, "qpos_off": self.qpos_off, "qpos_idx": self.qpos_idx,
+                 "frame_map": self.frame_map}
+            self.dev = DeviceIndex(a, device, staging)
+        return self.dev
+
+    def attn(self, dev):
+        return self.seq.attn(dev, "")
+
+
 PLAN_KEY = "_hero_plan"
+QA_PLAN_KEY = "_hero_qa_plan"
 _REPR_KEYS = ("f_attn_masks", "f_gather_index", "c_attn_masks", "num_subs", "sub_idx2frame_idx")
 
 
@@ -425,10 +485,12 @@ def plan_inputs(batch, kind="repr"):
         v = batch.get(key) if hasattr(batch, "get") else None
         return None if v is None else _np(v)
 
-    if kind != "repr":
+    if kind not in ("repr", "videoqa"):
         return {"attn_masks": _np(batch["attn_masks"]), "pos_ids": opt("pos_ids"),
                 "input_ids": opt("input_ids")}
     d = {k: (_np(batch[k]) if torch.is_tensor(batch[k]) else batch[k]) for k in _REPR_KEYS}
+    if kind == "videoqa":
+        d["_qa"] = qa_plan_inputs(batch)
     d["f_sub_pos_ids"] = opt("f_sub_pos_ids")
     d["f_sub_input_ids"] = opt("f_sub_input_ids")
     d["f_v_pos_ids"] = opt("f_v_pos_ids")
@@ -439,8 +501,11 @@ def plan_inputs(batch, kind="repr"):
 
 def build_plans(repr_in, txt_in=None):
     """ReprPlan (+ TxtPlan and the JointPlan of the fused video+query pass) from `plan_inputs`
-    dicts. Pure numpy: runs in collate workers / PlanPool processes."""
+    dicts. Pure numpy: runs in collate workers / PlanPool processes. A video QA batch's QaPlan
+    rides along as `rplan._qa` (PlanPool.attach stores it under QA_PLAN_KEY)."""
     rplan = ReprPlan(repr_in)
+    if repr_in.get("_qa") is not None:
+        rplan.__dict__["_qa"] = QaPlan(**repr_in["_qa"])
     if txt_in is None:
         return rplan, None
     tplan = TxtPlan(txt_in["attn_masks"], pos_ids=txt_in.get("pos_ids"),
@@ -461,13 +526,16 @@ class PlanPool:
         self._ex = cf.ProcessPoolExecutor(max_workers=workers, mp_context=mp.get_context("spawn"))
 
     def submit(self, batch, txt_batch=None):
-        return self._ex.submit(build_plans, plan_inputs(batch),
+        return self._ex.submit(build_plans, plan_inputs(batch, video_kind(batch)),
                                None if txt_batch is None else plan_inputs(txt_batch, "txt"))
 
     @staticmethod
     def attach(future, batch, txt_batch=None):
         rplan, tplan = future.result()
         batch[PLAN_KEY] = rplan
+        qplan = rplan.__dict__.pop("_qa", None)
+        if qplan is not None:
+            batch[QA_PLAN_KEY] = qplan
         if txt_batch is not None:
             txt_batch[PLAN_KEY] = tplan
         return batch, txt_batch
@@ -482,9 +550,11 @@ QUERY_PLAN_KEY = "_hero_query_plan"
 def attach_plan(batch, kind="repr"):
     """Collate-side hook: build the plan from HOST tensors (no device sync later) and stash it in
     the batch dict; `move_to_cuda`-style helpers leave non-tensor values alone.
-    kind: 'repr' (video batch), 'txt' (query batch), or 'vsm' — a VSM / VCMR training batch that
+    kind: 'repr' (video batch), 'txt' (query batch), 'vsm' — a VSM / VCMR training batch that
     carries its queries as `query_input_ids / query_pos_ids / query_attn_masks` (data/vcmr.py):
-    attaches the video plan, the query plan (QUERY_PLAN_KEY) and their joint plan.
+    attaches the video plan, the query plan (QUERY_PLAN_KEY) and their joint plan — or 'videoqa'
+    (data/videoQA.py video_qa_collate): the video plan of the cross-modal rows and the QaPlan of
+    the query-fused temporal rows (QA_PLAN_KEY).
     The plan captures the batch's token / position ids per packed token (FPlan.gather_ids): attach
     it AFTER any masking of `input_ids` (the reference masks in the dataset, before collate), and
     attach again if the ids are edited afterwards."""
@@ -495,6 +565,10 @@ def attach_plan(batch, kind="repr"):
         rplan.__dict__["_joint"] = JointPlan(rplan, tplan)
         batch[PLAN_KEY], batch[QUERY_PLAN_KEY] = rplan, tplan
         return batch
+    if kind == "videoqa":
+        batch[PLAN_KEY] = ReprPlan(batch)
+        batch[QA_PLAN_KEY] = qa_plan(batch)
+        return batch
     if kind == "repr":
         batch[PLAN_KEY] = ReprPlan(batch)
     else:
@@ -502,3 +576,34 @@ def attach_plan(batch, kind="repr"):
         batch[PLAN_KEY] = TxtPlan(batch["attn_masks"], pos_ids=get("pos_ids"),
                                   input_ids=get("input_ids"))
     return batch
+
+
+_QA_KEYS = ("c_attn_masks", "qa_attn_masks", "qa_input_ids", "qa_pos_ids")
+
+
+def video_kind(batch):
+    """'videoqa' for a video_qa_collate batch (it carries question / answer rows), else 'repr'."""
+    has = batch.get("qa_attn_masks") if hasattr(batch, "get") else None
+    return "videoqa" if has is not None else "repr"
+
+
+def qa_plan_inputs(batch):
+    """QaPlan arguments of a video_qa_collate batch as host arrays (`targets` gives the number of
+    videos). Tensors that live on the device come back in ONE device->host copy."""
+    ts = [batch[k] for k in _QA_KEYS]
+    dev = next((t.device for t in ts if torch.is_tensor(t) and t.device.type != "cpu"), None)
+    if dev is None:
+        arrays = [_np(t) for t in ts]
+    else:
+        parts = [torch.as_tensor(t).to(dev).reshape(-1).to(torch.int64) for t in ts]
+        flat = torch.cat(parts).cpu().numpy()
+        offs = np.cumsum([0] + [p.numel() for p in parts])
+        arrays = [flat[o:e].reshape(tuple(t.shape)) for o, e, t in zip(offs[:-1], offs[1:], ts)]
+    d = dict(zip(("c_attn_masks", "qa_attn_masks", "qa_input_ids", "qa_pos_ids"), arrays))
+    d["n_videos"] = int(batch["targets"].shape[0])
+    return d
+
+
+def qa_plan(batch):
+    """QaPlan of a video_qa_collate batch."""
+    return QaPlan(**qa_plan_inputs(batch))

@@ -257,3 +257,57 @@ def syn_vsm_batch(vb, qb, seed=0):
     b.update(query_input_ids=qb["input_ids"], query_pos_ids=qb["pos_ids"],
              query_attn_masks=qb["attn_masks"], targets=torch.tensor(tg, dtype=torch.long))
     return b
+
+
+def syn_videoqa_batch(n_videos=4, n_cand=5, seed=77, t_range=(40, 100), s_range=(8, 30),
+                      l_range=(4, 40), qa_range=(20, 60), vfeat_dim=VFEAT_DIM, vocab=50265,
+                      no_target=(), no_ts=()):
+    """data/videoQA.py:62-182 (VideoQaDataset.__getitem__ + video_qa_collate): per video one
+    question and `n_cand` answers; every (video, candidate) pair is one clip item of
+    `video_collate` whose subtitles are each followed by [SEP] q [SEP] a, so the rows are
+    video-major. `qa_input_ids / qa_pos_ids / qa_attn_masks` hold [SEP] q [SEP] a per candidate
+    (txt_input_collate), `targets` (Nv, 1) the answer index and `ts_targets` (Nv, 2) the start /
+    end frame; the videos listed in `no_target` / `no_ts` get -1 there. QA strings are
+    `qa_range` tokens long in total."""
+    gen = torch.Generator().manual_seed(seed)
+    rnd = random.Random(seed)
+    items, qa_ids, targets, ts = [], [], [], []
+    for v in range(n_videos):
+        T = rnd.randint(*t_range)
+        S = min(rnd.randint(*s_range), T)
+        cuts = sorted(rnd.sample(range(1, T), S - 1)) if S > 1 else []
+        bounds = [0] + cuts + [T]
+        groups = [list(range(bounds[s], bounds[s + 1])) for s in range(len(bounds) - 1)]
+        clip = make_clip(gen, T, groups, [rnd.randint(*l_range) for _ in groups], vfeat_dim,
+                         vocab)
+        n_q = rnd.randint(4, max(4, qa_range[0] // 2))
+        question = torch.randint(3, vocab, (n_q,), generator=gen)
+        for _ in range(n_cand):
+            n_a = max(1, rnd.randint(*qa_range) - n_q - 2)
+            answer = torch.randint(3, vocab, (n_a,), generator=gen)
+            qa = torch.cat([torch.tensor([SEP]), question, torch.tensor([SEP]), answer])
+            qa_ids.append(qa)
+            items.append({"feats": clip["feats"], "sub2frames": clip["sub2frames"],
+                          "subs": [torch.cat([s, qa]) for s in clip["subs"]]})
+        targets.append(-1 if v in no_target else rnd.randrange(n_cand))
+        st = rnd.randrange(0, T - 1)
+        ts.append((-1, -1) if v in no_ts else (st, min(T - 1, st + rnd.randint(1, 10))))
+    b = video_batch(items)
+    q = max(len(x) for x in qa_ids)
+    ids = torch.full((len(qa_ids), q), PAD, dtype=torch.long)
+    masks = torch.zeros(len(qa_ids), q, dtype=torch.long)
+    for i, x in enumerate(qa_ids):
+        ids[i, :len(x)] = x
+        masks[i, :len(x)] = 1
+    b["qa_input_ids"], b["qa_attn_masks"] = ids, masks
+    b["qa_pos_ids"] = torch.arange(q, dtype=torch.long).clamp(max=511).unsqueeze(0)
+    b["targets"] = torch.tensor(targets, dtype=torch.long).unsqueeze(1)
+    b["ts_targets"] = torch.tensor(ts, dtype=torch.long)
+    return b
+
+
+def syn_tvqa(seed=77, vfeat_dim=VFEAT_DIM):
+    """TVQA-shaped training batch of one GPU (config/train-tvqa-8gpu.json: train_batch_size 4):
+    4 videos x 5 candidates, clips of 40-100 frames, QA strings of 20-60 tokens (joint rows of
+    60-160 tokens, so some take the long-row attention path)."""
+    return syn_videoqa_batch(n_videos=4, n_cand=5, seed=seed, vfeat_dim=vfeat_dim)

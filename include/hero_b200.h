@@ -501,6 +501,33 @@ int hero_temporal_nms(const float* score, const int32_t* mom, int32_t nq, int32_
                       int32_t n_in, double thd, double interval, int32_t by_clip, int32_t n_out,
                       float* out_score, int32_t* out_mom, void* stream);
 
+/* ---- video QA attention pooling (hero_b200/csrc/qa.cu) ----
+ * model/videoQA.py:36-59,90-95 (get_modularized_video and its call): the two poolings of the
+ * temporal transformer's frame outputs. Rows r = (v*Nq + q)*L + l of map / mask / a / b index
+ * (video v, candidate q, frame l); h[v,q,l] is row map[r] of the packed fp32 outputs h [*, H], or
+ * zeros where map[r] < 0. With mask_logits(x, m) = x*m + (1-m)*(-1e4) in fp32:
+ *   a[v,q,l] = softmax over l of mask_logits(w_qa . h[v,q,l], m[r]),  qa_pooled [Nv*Nq, H] = sum_l a h
+ *   b[v,q,l] = softmax over q of mask_logits(w_st . h[v,q,l], m[r]),  st_pooled [Nv*L, H]  = sum_q b h
+ * The second softmax runs over the candidates (the reference's dim=1); masks may differ between
+ * the candidates of a video. a and b (fp32 [Nv*Nq*L]) are written for the backward.
+ * Bounds: 1 <= Nq <= 16, 1 <= L <= 512, H a positive multiple of 8, Nv >= 1; h, w_qa, w_st, the
+ * pooled tensors, their gradients and dh 16-byte aligned. Two launches forward, four backward. */
+int hero_qa_pool_fwd(const float* h, const int32_t* map, const float* mask, const float* w_qa,
+                     const float* w_st, int32_t Nv, int32_t Nq, int32_t L, int32_t H, float* a,
+                     float* b, float* qa_pooled, float* st_pooled, void* stream);
+/* fp32 elements of the scratch buffer hero_qa_pool_bwd needs:
+ * 4 R + 2 H ceil(R / 64) with R = Nv*Nq*L. */
+int64_t hero_qa_pool_bwd_scratch_floats(int32_t Nv, int32_t Nq, int32_t L, int32_t H);
+/* Backward of hero_qa_pool_fwd (same bounds and the same model/videoQA.py:36-59,90-95
+ * expressions). Writes d h into the rows map[r] >= 0 of dh (every other row is left untouched: the
+ * caller zero-fills the question / answer rows) and ACCUMULATES d w_qa, d w_st (fp32 [H]). The
+ * weight gradients are reduced in a fixed order without atomics: results are bitwise
+ * reproducible run to run. */
+int hero_qa_pool_bwd(const float* h, const int32_t* map, const float* mask, const float* w_qa,
+                     const float* w_st, const float* a, const float* b, const float* d_qa_pooled,
+                     const float* d_st_pooled, int32_t Nv, int32_t Nq, int32_t L, int32_t H,
+                     float* scratch, float* dh, float* dw_qa, float* dw_st, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
