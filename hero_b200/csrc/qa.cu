@@ -9,6 +9,10 @@
 // (padded frames are never computed in the packed layout). mask_logits(x, m) = x*m + (1-m)*(-1e4)
 // is evaluated with every operation rounded in fp32, as torch does. Everything is fp32 with fixed
 // reduction orders, so forward and backward are deterministic (no atomics).
+//
+// Every kernel takes a compile-time TWO: true computes both poolings (video QA); false computes
+// only the softmax over l and qa_pooled, the single pooling of VIOLIN (model/violin.py:30-47),
+// and never touches b, st_pooled or their gradients.
 #include "common.h"
 #include "ptx.cuh"
 
@@ -45,7 +49,8 @@ __device__ __forceinline__ float block_max(float v, float* red) {
   return warp_max(t);
 }
 
-// Two dot products of one H-row with two H-vectors, one warp, float4 loads, fixed order.
+// Dot products of one H-row with u (and with w when TWO), one warp, float4 loads, fixed order.
+template <bool TWO>
 __device__ __forceinline__ void warp_dot2(const float* __restrict__ row, const float* __restrict__ u,
                                           const float* __restrict__ w, int H, float& du,
                                           float& dw) {
@@ -54,16 +59,21 @@ __device__ __forceinline__ void warp_dot2(const float* __restrict__ row, const f
   for (int c = lane * 4; c < H; c += 128) {
     const float4 x = *reinterpret_cast<const float4*>(row + c);
     const float4 a = *reinterpret_cast<const float4*>(u + c);
-    const float4 b = *reinterpret_cast<const float4*>(w + c);
-    su += x.x * a.x + x.y * a.y + x.z * a.z + x.w * a.w;
-    sw += x.x * b.x + x.y * b.y + x.z * b.z + x.w * b.w;
+    if constexpr (TWO) {
+      const float4 b = *reinterpret_cast<const float4*>(w + c);
+      su += x.x * a.x + x.y * a.y + x.z * a.z + x.w * a.w;
+      sw += x.x * b.x + x.y * b.y + x.z * b.z + x.w * b.w;
+    } else {
+      su += x.x * a.x + x.y * a.y + x.z * a.z + x.w * a.w;
+    }
   }
   du = warp_sum(su);
-  dw = warp_sum(sw);
+  if constexpr (TWO) dw = warp_sum(sw);
 }
 
 // ---- forward ------------------------------------------------------------------------------------
 // One warp per (v,q,l) row: masked logits of both poolings into la / lb.
+template <bool TWO>
 __global__ void __launch_bounds__(QA_THREADS)
 qa_logits_kernel(const float* __restrict__ h, const int32_t* __restrict__ map,
                  const float* __restrict__ mask, const float* __restrict__ w_qa,
@@ -75,17 +85,19 @@ qa_logits_kernel(const float* __restrict__ h, const int32_t* __restrict__ map,
   if (row >= R) return;
   const int src = map[row];
   float sa = 0.f, sb = 0.f;
-  if (src >= 0) warp_dot2(h + (long long)src * H, w_qa, w_st, H, sa, sb);
+  if (src >= 0) warp_dot2<TWO>(h + (long long)src * H, w_qa, w_st, H, sa, sb);
   if ((threadIdx.x & 31) == 0) {
     const float m = mask[row];
     la[row] = qa_mask_logits(sa, m);
-    lb[row] = qa_mask_logits(sb, m);
+    if constexpr (TWO) lb[row] = qa_mask_logits(sb, m);
   }
 }
 
 // Blocks [0, Nv*Nq): softmax over l of one (v,q) and its qa-pooled row. Blocks [Nv*Nq, Nv*Nq +
 // Nv*L): softmax over q of one (v,l) and its st/ed-pooled row. la / lb are overwritten in place
-// with the probabilities (each element belongs to exactly one block).
+// with the probabilities (each element belongs to exactly one block). Single pooling: only the
+// first Nv*Nq blocks are launched.
+template <bool TWO>
 __global__ void __launch_bounds__(QA_THREADS)
 qa_pool_kernel(const float* __restrict__ h, const int32_t* __restrict__ map, int Nv, int Nq,
                int L, int H, float* __restrict__ pa, float* __restrict__ pb,
@@ -99,7 +111,7 @@ qa_pool_kernel(const float* __restrict__ h, const int32_t* __restrict__ map, int
   const int nvq = Nv * Nq;
   int n;
   float* out;
-  if ((int)blockIdx.x < nvq) {
+  if (!TWO || (int)blockIdx.x < nvq) {
     const int vq = blockIdx.x;
     float* lg = pa + (long long)vq * L;
     float mx = -INFINITY;
@@ -161,6 +173,7 @@ qa_pool_kernel(const float* __restrict__ h, const int32_t* __restrict__ map, int
 
 // ---- backward -----------------------------------------------------------------------------------
 // One warp per row: da = d qa_pooled[v,q] . h, db = d st_pooled[v,l] . h.
+template <bool TWO>
 __global__ void __launch_bounds__(QA_THREADS)
 qa_bwd_dots_kernel(const float* __restrict__ h, const int32_t* __restrict__ map,
                    const float* __restrict__ dqa, const float* __restrict__ dst, int Nq, int L,
@@ -173,16 +186,17 @@ qa_bwd_dots_kernel(const float* __restrict__ h, const int32_t* __restrict__ map,
   const int vq = row / L, l = row % L, v = vq / Nq;
   float sa = 0.f, sb = 0.f;
   if (src >= 0)
-    warp_dot2(h + (long long)src * H, dqa + (long long)vq * H, dst + ((long long)v * L + l) * H,
-              H, sa, sb);
+    warp_dot2<TWO>(h + (long long)src * H, dqa + (long long)vq * H,
+                   TWO ? dst + ((long long)v * L + l) * H : nullptr, H, sa, sb);
   if ((threadIdx.x & 31) == 0) {
     da[row] = sa;
-    db[row] = sb;
+    if constexpr (TWO) db[row] = sb;
   }
 }
 
 // One block per (v,q): softmax backward of both poolings (d logit, times the mask_logits slope
 // m) into gqa / gst, and d h of its frame rows.
+template <bool TWO>
 __global__ void __launch_bounds__(QA_THREADS, 1)
 qa_bwd_rows_kernel(const int32_t* __restrict__ map, const float* __restrict__ mask,
                    const float* __restrict__ pa, const float* __restrict__ pb,
@@ -202,80 +216,96 @@ qa_bwd_rows_kernel(const int32_t* __restrict__ map, const float* __restrict__ ma
   for (int l = warp; l < L; l += QA_WARPS) {
     const long long row = r0 + l;
     const float m = mask[row];
-    const float a = pa[row], b = pb[row];
+    const float a = pa[row];
     const float ga = a * (da[row] - s) * m;
-    float t = 0.f;                          // sum_q' b db over the candidates of (v, l)
-    const float* pbl = pb + (long long)v * Nq * L + l;
-    const float* dbl = db + (long long)v * Nq * L + l;
+    float b = 0.f, gb = 0.f;
+    if constexpr (TWO) {
+      b = pb[row];
+      float t = 0.f;                        // sum_q' b db over the candidates of (v, l)
+      const float* pbl = pb + (long long)v * Nq * L + l;
+      const float* dbl = db + (long long)v * Nq * L + l;
 #pragma unroll 1
-    for (int q = 0; q < Nq; ++q) t += pbl[q * L] * dbl[q * L];
-    const float gb = b * (db[row] - t) * m;
+      for (int q = 0; q < Nq; ++q) t += pbl[q * L] * dbl[q * L];
+      gb = b * (db[row] - t) * m;
+    }
     if (lane == 0) {
       gqa[row] = ga;
-      gst[row] = gb;
+      if constexpr (TWO) gst[row] = gb;
     }
     const int src = map[row];
     if (src < 0) continue;
     const float* dq = dqa + (long long)vq * H;
-    const float* ds = dst + ((long long)v * L + l) * H;
+    const float* ds = TWO ? dst + ((long long)v * L + l) * H : nullptr;
     float* out = dh + (long long)src * H;
     for (int c = lane * 4; c < H; c += 128) {
       const float4 x = *reinterpret_cast<const float4*>(dq + c);
-      const float4 y = *reinterpret_cast<const float4*>(ds + c);
       const float4 u = *reinterpret_cast<const float4*>(w_qa + c);
-      const float4 w = *reinterpret_cast<const float4*>(w_st + c);
       float4 o;
-      o.x = a * x.x + ga * u.x + b * y.x + gb * w.x;
-      o.y = a * x.y + ga * u.y + b * y.y + gb * w.y;
-      o.z = a * x.z + ga * u.z + b * y.z + gb * w.z;
-      o.w = a * x.w + ga * u.w + b * y.w + gb * w.w;
+      if constexpr (TWO) {
+        const float4 y = *reinterpret_cast<const float4*>(ds + c);
+        const float4 w = *reinterpret_cast<const float4*>(w_st + c);
+        o.x = a * x.x + ga * u.x + b * y.x + gb * w.x;
+        o.y = a * x.y + ga * u.y + b * y.y + gb * w.y;
+        o.z = a * x.z + ga * u.z + b * y.z + gb * w.z;
+        o.w = a * x.w + ga * u.w + b * y.w + gb * w.w;
+      } else {
+        o.x = a * x.x + ga * u.x;
+        o.y = a * x.y + ga * u.y;
+        o.z = a * x.z + ga * u.z;
+        o.w = a * x.w + ga * u.w;
+      }
       *reinterpret_cast<float4*>(out + c) = o;
     }
   }
 }
 
-// Partial weight gradients over QA_CHUNK_ROWS rows: part[chunk][0|1][c] = sum_rows g * h[row][c].
+// Partial weight gradients over QA_CHUNK_ROWS rows: part[chunk][0|1][c] = sum_rows g * h[row][c]
+// (single pooling: part[chunk][0][c] only).
+template <bool TWO>
 __global__ void __launch_bounds__(QA_THREADS)
 qa_bwd_wpart_kernel(const float* __restrict__ h, const int32_t* __restrict__ map,
                     const float* __restrict__ gqa, const float* __restrict__ gst, int R, int H,
                     float* __restrict__ part) {
+  constexpr int NP = TWO ? 2 : 1;
   pdl_wait();
   pdl_launch_dependents();
-  __shared__ float sg[2][QA_CHUNK_ROWS];
+  __shared__ float sg[NP][QA_CHUNK_ROWS];
   __shared__ int32_t ssrc[QA_CHUNK_ROWS];
   const int tid = threadIdx.x;
   const int r0 = blockIdx.x * QA_CHUNK_ROWS;
   const int nr = min(QA_CHUNK_ROWS, R - r0);
   if (tid < nr) {
     sg[0][tid] = gqa[r0 + tid];
-    sg[1][tid] = gst[r0 + tid];
+    if constexpr (TWO) sg[1][tid] = gst[r0 + tid];
     ssrc[tid] = map[r0 + tid];
   }
   __syncthreads();
-  float* p0 = part + (long long)blockIdx.x * 2 * H;
+  float* p0 = part + (long long)blockIdx.x * NP * H;
   for (int c = tid; c < H; c += QA_THREADS) {
     float a = 0.f, b = 0.f;
     for (int i = 0; i < nr; ++i) {
       if (ssrc[i] < 0) continue;
       const float x = h[(long long)ssrc[i] * H + c];
       a += sg[0][i] * x;
-      b += sg[1][i] * x;
+      if constexpr (TWO) b += sg[1][i] * x;
     }
     p0[c] = a;
-    p0[H + c] = b;
+    if constexpr (TWO) p0[H + c] = b;
   }
 }
 
 // dw_qa[c] += sum over chunks (in order) of part[chunk][0][c]; dw_st likewise.
+template <bool TWO>
 __global__ void __launch_bounds__(QA_THREADS)
 qa_bwd_wsum_kernel(const float* __restrict__ part, int n_chunks, int H, float* __restrict__ dw_qa,
                    float* __restrict__ dw_st) {
+  constexpr int NP = TWO ? 2 : 1;
   pdl_wait();
   pdl_launch_dependents();
   const int c = blockIdx.x * QA_THREADS + threadIdx.x;
-  if (c >= 2 * H) return;
+  if (c >= NP * H) return;
   float s = 0.f;
-  for (int k = 0; k < n_chunks; ++k) s += part[(long long)k * 2 * H + c];
+  for (int k = 0; k < n_chunks; ++k) s += part[(long long)k * NP * H + c];
   if (c < H)
     dw_qa[c] += s;
   else
@@ -293,6 +323,40 @@ static int qa_check(const void* h, int Nv, int Nq, int L, int H) {
   return HERO_OK;
 }
 
+// The two forward launches; the single pooling launches no softmax-over-q blocks.
+template <bool TWO>
+static int qa_fwd_launch(const float* h, const int32_t* map, const float* mask, const float* w_qa,
+                         const float* w_st, int Nv, int Nq, int L, int H, int R, float* a, float* b,
+                         float* qa_pooled, float* st_pooled, cudaStream_t s) {
+  HERO_CUDA_CHECK(launch_pdl(qa_logits_kernel<TWO>, dim3(ceil_div(R, QA_WARPS)), dim3(QA_THREADS),
+                             0, s, h, map, mask, w_qa, w_st, R, H, a, b));
+  HERO_CUDA_CHECK(launch_pdl(qa_pool_kernel<TWO>, dim3(Nv * Nq + (TWO ? Nv * L : 0)),
+                             dim3(QA_THREADS), 0, s, h, map, Nv, Nq, L, H, a, b, qa_pooled,
+                             st_pooled));
+  return HERO_OK;
+}
+
+// The four backward launches; part holds TWO ? 2 : 1 partial rows of H per chunk.
+template <bool TWO>
+static int qa_bwd_launch(const float* h, const int32_t* map, const float* mask, const float* w_qa,
+                         const float* w_st, const float* a, const float* b, const float* d_qa_pooled,
+                         const float* d_st_pooled, int Nv, int Nq, int L, int H, int R,
+                         int n_chunks, float* da, float* db, float* gqa, float* gst, float* part,
+                         float* dh, float* dw_qa, float* dw_st, cudaStream_t s) {
+  HERO_CUDA_CHECK(launch_pdl(qa_bwd_dots_kernel<TWO>, dim3(ceil_div(R, QA_WARPS)),
+                             dim3(QA_THREADS), 0, s, h, map, d_qa_pooled, d_st_pooled, Nq, L, R, H,
+                             da, db));
+  HERO_CUDA_CHECK(launch_pdl(qa_bwd_rows_kernel<TWO>, dim3(Nv * Nq), dim3(QA_THREADS), 0, s, map,
+                             mask, a, b, (const float*)da, (const float*)db, d_qa_pooled,
+                             d_st_pooled, w_qa, w_st, Nq, L, H, gqa, gst, dh));
+  HERO_CUDA_CHECK(launch_pdl(qa_bwd_wpart_kernel<TWO>, dim3(n_chunks), dim3(QA_THREADS), 0, s, h,
+                             map, (const float*)gqa, (const float*)gst, R, H, part));
+  HERO_CUDA_CHECK(launch_pdl(qa_bwd_wsum_kernel<TWO>, dim3(ceil_div((TWO ? 2 : 1) * H, QA_THREADS)),
+                             dim3(QA_THREADS), 0, s, (const float*)part, n_chunks, H, dw_qa,
+                             dw_st));
+  return HERO_OK;
+}
+
 }  // namespace hero
 
 using namespace hero;
@@ -301,8 +365,10 @@ extern "C" int hero_qa_pool_fwd(const float* h, const int32_t* map, const float*
                                 const float* w_qa, const float* w_st, int32_t Nv, int32_t Nq,
                                 int32_t L, int32_t H, float* a, float* b, float* qa_pooled,
                                 float* st_pooled, void* stream) {
-  HERO_REQUIRE(h && map && mask && w_qa && w_st && a && b && qa_pooled && st_pooled,
-               "qa_pool_fwd: null pointer");
+  HERO_REQUIRE(h && map && mask && w_qa && a && qa_pooled, "qa_pool_fwd: null pointer");
+  const bool two = w_st != nullptr;
+  HERO_REQUIRE((b != nullptr) == two && (st_pooled != nullptr) == two,
+               "qa_pool_fwd: w_st, b and st_pooled must be all set or all NULL");
   int st = qa_check(h, Nv, Nq, L, H);
   if (st != HERO_OK) return st;
   HERO_REQUIRE(qa_aligned(h) && qa_aligned(w_qa) && qa_aligned(w_st) && qa_aligned(qa_pooled) &&
@@ -310,11 +376,11 @@ extern "C" int hero_qa_pool_fwd(const float* h, const int32_t* map, const float*
                "qa_pool_fwd: h, w_qa, w_st and the pooled outputs must be 16-byte aligned");
   const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const int R = Nv * Nq * L;
-  HERO_CUDA_CHECK(launch_pdl(qa_logits_kernel, dim3(ceil_div(R, QA_WARPS)), dim3(QA_THREADS), 0, s,
-                             h, map, mask, w_qa, w_st, R, (int)H, a, b));
-  HERO_CUDA_CHECK(launch_pdl(qa_pool_kernel, dim3(Nv * Nq + Nv * L), dim3(QA_THREADS), 0, s, h, map,
-                             (int)Nv, (int)Nq, (int)L, (int)H, a, b, qa_pooled, st_pooled));
-  return HERO_OK;
+  if (two)
+    return qa_fwd_launch<true>(h, map, mask, w_qa, w_st, Nv, Nq, L, H, R, a, b, qa_pooled,
+                               st_pooled, s);
+  return qa_fwd_launch<false>(h, map, mask, w_qa, w_st, Nv, Nq, L, H, R, a, b, qa_pooled,
+                              st_pooled, s);
 }
 
 extern "C" int64_t hero_qa_pool_bwd_scratch_floats(int32_t Nv, int32_t Nq, int32_t L, int32_t H) {
@@ -328,9 +394,11 @@ extern "C" int hero_qa_pool_bwd(const float* h, const int32_t* map, const float*
                                 const float* d_st_pooled, int32_t Nv, int32_t Nq, int32_t L,
                                 int32_t H, float* scratch, float* dh, float* dw_qa, float* dw_st,
                                 void* stream) {
-  HERO_REQUIRE(h && map && mask && w_qa && w_st && a && b && d_qa_pooled && d_st_pooled &&
-                   scratch && dh && dw_qa && dw_st,
+  HERO_REQUIRE(h && map && mask && w_qa && a && d_qa_pooled && scratch && dh && dw_qa,
                "qa_pool_bwd: null pointer");
+  const bool two = w_st != nullptr;
+  HERO_REQUIRE((b != nullptr) == two && (d_st_pooled != nullptr) == two && (dw_st != nullptr) == two,
+               "qa_pool_bwd: w_st, b, d_st_pooled and dw_st must be all set or all NULL");
   int st = qa_check(h, Nv, Nq, L, H);
   if (st != HERO_OK) return st;
   HERO_REQUIRE(qa_aligned(h) && qa_aligned(w_qa) && qa_aligned(w_st) && qa_aligned(d_qa_pooled) &&
@@ -344,16 +412,9 @@ extern "C" int hero_qa_pool_bwd(const float* h, const int32_t* map, const float*
   float* gqa = db + R;
   float* gst = gqa + R;
   float* part = gst + R;
-  HERO_CUDA_CHECK(launch_pdl(qa_bwd_dots_kernel, dim3(ceil_div(R, QA_WARPS)), dim3(QA_THREADS), 0,
-                             s, h, map, d_qa_pooled, d_st_pooled, (int)Nq, (int)L, R, (int)H, da,
-                             db));
-  HERO_CUDA_CHECK(launch_pdl(qa_bwd_rows_kernel, dim3(Nv * Nq), dim3(QA_THREADS), 0, s, map, mask,
-                             a, b, (const float*)da, (const float*)db, d_qa_pooled, d_st_pooled,
-                             w_qa, w_st, (int)Nq, (int)L, (int)H, gqa, gst, dh));
-  HERO_CUDA_CHECK(launch_pdl(qa_bwd_wpart_kernel, dim3(n_chunks), dim3(QA_THREADS), 0, s, h, map,
-                             (const float*)gqa, (const float*)gst, R, (int)H, part));
-  HERO_CUDA_CHECK(launch_pdl(qa_bwd_wsum_kernel, dim3(ceil_div(2 * H, QA_THREADS)),
-                             dim3(QA_THREADS), 0, s, (const float*)part, n_chunks, (int)H, dw_qa,
-                             dw_st));
-  return HERO_OK;
+  if (two)
+    return qa_bwd_launch<true>(h, map, mask, w_qa, w_st, a, b, d_qa_pooled, d_st_pooled, Nv, Nq,
+                               L, H, R, n_chunks, da, db, gqa, gst, part, dh, dw_qa, dw_st, s);
+  return qa_bwd_launch<false>(h, map, mask, w_qa, w_st, a, b, d_qa_pooled, d_st_pooled, Nv, Nq, L,
+                              H, R, n_chunks, da, db, gqa, gst, part, dh, dw_qa, dw_st, s);
 }

@@ -16,6 +16,7 @@
   the TVR recall metrics of utils/tvr_standalone_eval.py vectorised over queries on the host
   (DESIGN §4 "Temporal NMS and TVR metrics").
 * `validate_videoqa` — eval_videoQA.py:120-173 for one process on HeroForVideoQA.
+* `validate_violin` — eval_violin.py:118-164 for one process on HeroForViolin.
 * `ModelSaver` / `TrainingRestorer` — utils/save.py:112-181 with the same file layout (`vocab_padded`
   flag, `model_step_<n>.pt`, `train_state_<n>.pt`, `restore.pt` + backup), so checkpoints are
   interchangeable with the reference's; optimizer state is FusedAdamW's flat moments.
@@ -776,6 +777,49 @@ def validate_videoqa(model, loader, split, task="tvqa", save_logits=False):
         tot_time = time.time() - t0
         val_log = {"valid/loss": val_loss / n_ex, "valid/acc": tot_score / n_ex,
                    "valid/ex_per_s": n_ex / tot_time}
+    model.train()
+    return val_log, results, logits
+
+
+@torch.no_grad()
+def validate_violin(model, loader, split, save_logits=False):
+    """eval_violin.py:118-164 (validate_violin) for one process: returns (val_log, results, logits)
+    with `valid/{split}_loss` (summed binary cross entropy of sigmoid(score) over the examples),
+    `valid/{split}_acc` and `valid/{split}_ex_per_s`, results[str(qid)] = int(sigmoid(score) > 0.5)
+    and, with `save_logits`, logits[str(qid)] = [score]. Predictions, the loss sum and the correct
+    count are computed on the device; each batch makes one device->host copy. Unlike the
+    reference, a one-row batch works (there `predictions.squeeze().tolist()` is an int and the zip
+    over it raises). Averaging across ranks (all_gather_list) is left to the caller."""
+    import time
+    model.eval()
+    val_loss, n_ex, tot_score = 0.0, 0, 0
+    results, logits = {}, {}
+    t0 = time.time()
+    for batch in loader:
+        qids = batch.pop("qids")
+        scores = model(batch, "violin", compute_loss=False)             # (rows, 1)
+        tgt = batch["targets"].to(scores.device).reshape(scores.shape)
+        probs = torch.sigmoid(scores)
+        predictions = (probs > 0.5).long()
+        loss = torch.nn.functional.binary_cross_entropy(probs, tgt.to(scores.dtype),
+                                                        reduction="sum")
+        correct = (predictions == tgt).sum()
+        packed = torch.cat([predictions.float().reshape(-1), loss.reshape(1).float(),
+                            correct.reshape(1).float()] +
+                           ([scores.float().reshape(-1)] if save_logits else []))
+        host = packed.cpu()
+        n = predictions.numel()
+        for qid, answer in zip(qids, host[:n].long().tolist()):
+            results[str(qid)] = answer
+        if save_logits:
+            for qid, score in zip(qids, host[n + 2:].tolist()):
+                logits[str(qid)] = [score]
+        val_loss += float(host[n])
+        tot_score += int(host[n + 1])
+        n_ex += len(qids)
+    tot_time = time.time() - t0
+    val_log = {f"valid/{split}_loss": val_loss / n_ex, f"valid/{split}_acc": tot_score / n_ex,
+               f"valid/{split}_ex_per_s": n_ex / tot_time}
     model.train()
     return val_log, results, logits
 

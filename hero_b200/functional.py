@@ -11,6 +11,7 @@ gradients; the arithmetic reads the bf16 working copies held in `ctx_w` objects.
     frame_embed         FrameEmbeddings               model/embed.py:146-161
     qa_fused_embed      frame + question/answer embeddings of video QA  model/videoQA.py:68-78
     qa_pool             both attention poolings of video QA             model/videoQA.py:36-59
+                        (w_st=None: the single pooling of VIOLIN)       model/violin.py:30-47
     pack / unpack       padded <-> packed layouts
 """
 import torch
@@ -542,40 +543,46 @@ def qa_fused_embed(g, cfg, params):
 class _QaPool(torch.autograd.Function):
     """Both attention poolings of video QA (model/videoQA.py:36-59) on the packed fp32 temporal
     outputs h: qa_pooled (Nv*Nq, H) over the frames of each candidate, st_pooled (Nv*L, H) over
-    the candidates of each frame (csrc/qa.cu)."""
+    the candidates of each frame (csrc/qa.cu). With w_st None only qa_pooled is computed and
+    returned (VIOLIN, model/violin.py:30-47)."""
 
     @staticmethod
     def forward(ctx, h, w_qa, w_st, frame_map, mask, dims):
         nv, nq, length = dims
         H = h.shape[1]
         h = h.contiguous()
+        two = w_st is not None
         wq = w_qa.detach().float().reshape(-1).contiguous()
-        ws = w_st.detach().float().reshape(-1).contiguous()
+        ws = w_st.detach().float().reshape(-1).contiguous() if two else None
         mask = mask.float().reshape(-1).contiguous()
         a = torch.empty(nv * nq * length, dtype=F32, device=h.device)
-        b = torch.empty_like(a)
+        b = torch.empty_like(a) if two else None
         qa = torch.empty((nv * nq, H), dtype=F32, device=h.device)
-        sp = torch.empty((nv * length, H), dtype=F32, device=h.device)
+        sp = torch.empty((nv * length, H), dtype=F32, device=h.device) if two else None
         ops.qa_pool_fwd(h, frame_map, mask, wq, ws, nv, nq, length, a, b, qa, sp)
         ctx.st = (h, wq, ws, frame_map, mask, a, b, dims)
         ctx.w_shape = tuple(w_qa.shape)
-        return qa, sp
+        return (qa, sp) if two else qa
 
     @staticmethod
-    def backward(ctx, d_qa, d_st):
+    def backward(ctx, d_qa, d_st=None):
         h, wq, ws, frame_map, mask, a, b, (nv, nq, length) = ctx.st
+        two = ws is not None
         dh = torch.zeros_like(h)                 # question / answer rows get no gradient here
-        dwq, dws = torch.zeros_like(wq), torch.zeros_like(ws)
+        dwq, dws = torch.zeros_like(wq), (torch.zeros_like(ws) if two else None)
         z = lambda t, shape: torch.zeros(shape, dtype=F32, device=h.device) if t is None \
             else t.float().contiguous()
         ops.qa_pool_bwd(h, frame_map, mask, wq, ws, a, b, z(d_qa, (nv * nq, h.shape[1])),
-                        z(d_st, (nv * length, h.shape[1])), nv, nq, length, dh, dwq, dws)
+                        z(d_st, (nv * length, h.shape[1])) if two else None, nv, nq, length, dh,
+                        dwq, dws)
         ctx.st = None
-        return dh, dwq.view(ctx.w_shape), dws.view(ctx.w_shape), None, None, None
+        return (dh, dwq.view(ctx.w_shape), dws.view(ctx.w_shape) if two else None, None, None,
+                None)
 
 
 def qa_pool(h, w_qa, w_st, frame_map, mask, nv, nq, length):
     """h fp32 [n_tok, H]; frame_map int32 [Nv*Nq*L] (plan.QaPlan); mask [Nv*Nq*L] 0/1.
+    Returns (qa_pooled, st_pooled), or qa_pooled alone when w_st is None.
     Bounds (ValueError before any launch): Nq <= 16, L <= 512, H a multiple of 8."""
     ops._qa_bounds(nv, nq, length, h.shape[1])
     return _QaPool.apply(h, w_qa, w_st, frame_map, mask, (nv, nq, length))

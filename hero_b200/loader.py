@@ -69,7 +69,7 @@ class BatchStager:
                         joint.dev = None
                         joint.to(self.device, self._staging(bufs, (bi, "joint")))
                 qplan = d.get(QA_PLAN_KEY)
-                if qplan is not None:     # video QA: the query-fused rows' plan likewise
+                if qplan is not None:     # video QA / VIOLIN: the query-fused rows' plan likewise
                     qplan.dev = None
                     qplan.to(self.device, self._staging(bufs, (bi, "qa")))
                 out.append(d)
@@ -110,8 +110,8 @@ def record_plans(batches, stream):
 
 class PrefetchLoader:
     """data/loader.py:89-144 on a BatchStager. `loader` yields host batches: a dict (video batch,
-    'repr' plan; a video_qa_collate batch gets the 'videoqa' plans) or a (video_dict, query_dict)
-    pair for the fused `forward_repr_txt` path. Plans
+    'repr' plan; a video_qa_collate batch gets the 'videoqa' plans, a violin_collate batch the
+    'violin' ones) or a (video_dict, query_dict) pair for the fused `forward_repr_txt` path. Plans
     already attached by the collate function are used as they are; otherwise they are built two
     batches ahead in `plan_workers` processes (0: in this process)."""
 

@@ -662,12 +662,13 @@ def _qa_bounds(nv, nq, length, h):
 
 def qa_pool_fwd(h, frame_map, mask, w_qa, w_st, nv, nq, length, a, b, qa_pooled, st_pooled):
     """Both attention poolings of model/videoQA.py:36-59 over the packed fp32 rows h [*, H]:
-    a / b [Nv*Nq*L] pooling weights, qa_pooled [Nv*Nq, H], st_pooled [Nv*L, H] (`hero_qa_pool_fwd`)."""
+    a / b [Nv*Nq*L] pooling weights, qa_pooled [Nv*Nq, H], st_pooled [Nv*L, H] (`hero_qa_pool_fwd`).
+    w_st = b = st_pooled = None: the single pooling of model/violin.py:30-47 (a and qa_pooled)."""
     _require_cuda(h, frame_map, mask, w_qa, w_st, a, b, qa_pooled, st_pooled)
     H = h.shape[1]
     _qa_bounds(nv, nq, length, H)
     for t in (h, mask, w_qa, w_st, a, b, qa_pooled, st_pooled):
-        assert t.dtype == torch.float32 and t.is_contiguous()
+        assert t is None or (t.dtype == torch.float32 and t.is_contiguous())
     assert frame_map.dtype == torch.int32 and frame_map.numel() == nv * nq * length
     _count(2)
     _lib.check(_lib.lib().hero_qa_pool_fwd(_ptr(h), _ptr(frame_map), _ptr(mask), _ptr(w_qa),
@@ -678,12 +679,12 @@ def qa_pool_fwd(h, frame_map, mask, w_qa, w_st, nv, nq, length, a, b, qa_pooled,
 def qa_pool_bwd(h, frame_map, mask, w_qa, w_st, a, b, d_qa, d_st, nv, nq, length, dh, dw_qa,
                 dw_st):
     """Backward of qa_pool_fwd (`hero_qa_pool_bwd`): writes the frame rows of dh, accumulates
-    dw_qa / dw_st (fp32 [H]) in a fixed order."""
+    dw_qa / dw_st (fp32 [H]) in a fixed order. w_st = b = d_st = dw_st = None: single pooling."""
     _require_cuda(h, frame_map, mask, w_qa, w_st, a, b, d_qa, d_st, dh, dw_qa, dw_st)
     H = h.shape[1]
     _qa_bounds(nv, nq, length, H)
     for t in (h, mask, w_qa, w_st, a, b, d_qa, d_st, dh, dw_qa, dw_st):
-        assert t.dtype == torch.float32 and t.is_contiguous()
+        assert t is None or (t.dtype == torch.float32 and t.is_contiguous())
     n = _lib.lib().hero_qa_pool_bwd_scratch_floats(nv, nq, length, H)
     scratch = torch.empty(n, dtype=torch.float32, device=h.device)
     _count(4)

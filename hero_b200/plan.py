@@ -421,7 +421,10 @@ class QaPlan:
     column as temporal position; question / answer tokens take `qa_pos_ids`.
 
     Frame tokens appear in the same row-major order as CPlan's clip tokens, so frame k of the
-    packed stream reads row k of the cross-modal output `g` (no source map needed)."""
+    packed stream reads row k of the cross-modal output `g` (no source map needed).
+
+    VIOLIN (model/violin.py:50-70) has the same rows with a statement in place of question +
+    answer: built with n_videos = rows, so Nq = 1 and each statement row pools its own frames."""
 
     def __init__(self, c_attn_masks, qa_attn_masks, qa_input_ids, qa_pos_ids, n_videos):
         cm, qm = _np(c_attn_masks) != 0, _np(qa_attn_masks) != 0
@@ -485,12 +488,12 @@ def plan_inputs(batch, kind="repr"):
         v = batch.get(key) if hasattr(batch, "get") else None
         return None if v is None else _np(v)
 
-    if kind not in ("repr", "videoqa"):
+    if kind not in ("repr",) + tuple(_QA_PREFIX):
         return {"attn_masks": _np(batch["attn_masks"]), "pos_ids": opt("pos_ids"),
                 "input_ids": opt("input_ids")}
     d = {k: (_np(batch[k]) if torch.is_tensor(batch[k]) else batch[k]) for k in _REPR_KEYS}
-    if kind == "videoqa":
-        d["_qa"] = qa_plan_inputs(batch)
+    if kind in _QA_PREFIX:
+        d["_qa"] = qa_plan_inputs(batch, _QA_PREFIX[kind])
     d["f_sub_pos_ids"] = opt("f_sub_pos_ids")
     d["f_sub_input_ids"] = opt("f_sub_input_ids")
     d["f_v_pos_ids"] = opt("f_v_pos_ids")
@@ -501,8 +504,8 @@ def plan_inputs(batch, kind="repr"):
 
 def build_plans(repr_in, txt_in=None):
     """ReprPlan (+ TxtPlan and the JointPlan of the fused video+query pass) from `plan_inputs`
-    dicts. Pure numpy: runs in collate workers / PlanPool processes. A video QA batch's QaPlan
-    rides along as `rplan._qa` (PlanPool.attach stores it under QA_PLAN_KEY)."""
+    dicts. Pure numpy: runs in collate workers / PlanPool processes. A video QA or VIOLIN batch's
+    QaPlan rides along as `rplan._qa` (PlanPool.attach stores it under QA_PLAN_KEY)."""
     rplan = ReprPlan(repr_in)
     if repr_in.get("_qa") is not None:
         rplan.__dict__["_qa"] = QaPlan(**repr_in["_qa"])
@@ -553,8 +556,8 @@ def attach_plan(batch, kind="repr"):
     kind: 'repr' (video batch), 'txt' (query batch), 'vsm' — a VSM / VCMR training batch that
     carries its queries as `query_input_ids / query_pos_ids / query_attn_masks` (data/vcmr.py):
     attaches the video plan, the query plan (QUERY_PLAN_KEY) and their joint plan — or 'videoqa'
-    (data/videoQA.py video_qa_collate): the video plan of the cross-modal rows and the QaPlan of
-    the query-fused temporal rows (QA_PLAN_KEY).
+    (data/videoQA.py video_qa_collate) / 'violin' (data/violin.py violin_collate): the video plan
+    of the cross-modal rows and the QaPlan of the query-fused temporal rows (QA_PLAN_KEY).
     The plan captures the batch's token / position ids per packed token (FPlan.gather_ids): attach
     it AFTER any masking of `input_ids` (the reference masks in the dataset, before collate), and
     attach again if the ids are edited afterwards."""
@@ -565,9 +568,9 @@ def attach_plan(batch, kind="repr"):
         rplan.__dict__["_joint"] = JointPlan(rplan, tplan)
         batch[PLAN_KEY], batch[QUERY_PLAN_KEY] = rplan, tplan
         return batch
-    if kind == "videoqa":
+    if kind in _QA_PREFIX:
         batch[PLAN_KEY] = ReprPlan(batch)
-        batch[QA_PLAN_KEY] = qa_plan(batch)
+        batch[QA_PLAN_KEY] = qa_plan(batch, _QA_PREFIX[kind])
         return batch
     if kind == "repr":
         batch[PLAN_KEY] = ReprPlan(batch)
@@ -578,19 +581,27 @@ def attach_plan(batch, kind="repr"):
     return batch
 
 
-_QA_KEYS = ("c_attn_masks", "qa_attn_masks", "qa_input_ids", "qa_pos_ids")
+# key prefix of the query-fused text of each kind: question + answer rows of video QA, the
+# statement rows of VIOLIN
+_QA_PREFIX = {"videoqa": "qa", "violin": "q"}
 
 
 def video_kind(batch):
-    """'videoqa' for a video_qa_collate batch (it carries question / answer rows), else 'repr'."""
-    has = batch.get("qa_attn_masks") if hasattr(batch, "get") else None
-    return "videoqa" if has is not None else "repr"
+    """'videoqa' for a video_qa_collate batch (it carries question / answer rows), 'violin' for a
+    violin_collate batch (statement rows), else 'repr'."""
+    get = batch.get if hasattr(batch, "get") else (lambda k: None)
+    for kind, prefix in _QA_PREFIX.items():
+        if get(f"{prefix}_attn_masks") is not None:
+            return kind
+    return "repr"
 
 
-def qa_plan_inputs(batch):
-    """QaPlan arguments of a video_qa_collate batch as host arrays (`targets` gives the number of
-    videos). Tensors that live on the device come back in ONE device->host copy."""
-    ts = [batch[k] for k in _QA_KEYS]
+def qa_plan_inputs(batch, prefix="qa"):
+    """QaPlan arguments of a batch whose query-fused text is `{prefix}_attn_masks / _input_ids /
+    _pos_ids`, as host arrays. `targets` gives the number of videos: (Nv, 1) in video QA, one row
+    per statement in VIOLIN. Tensors that live on the device come back in ONE device->host copy."""
+    ts = [batch[k] for k in ("c_attn_masks", f"{prefix}_attn_masks", f"{prefix}_input_ids",
+                             f"{prefix}_pos_ids")]
     dev = next((t.device for t in ts if torch.is_tensor(t) and t.device.type != "cpu"), None)
     if dev is None:
         arrays = [_np(t) for t in ts]
@@ -604,6 +615,6 @@ def qa_plan_inputs(batch):
     return d
 
 
-def qa_plan(batch):
-    """QaPlan of a video_qa_collate batch."""
-    return QaPlan(**qa_plan_inputs(batch))
+def qa_plan(batch, prefix="qa"):
+    """QaPlan of a video_qa_collate batch (prefix "qa") or a violin_collate batch ("q")."""
+    return QaPlan(**qa_plan_inputs(batch, prefix))

@@ -311,3 +311,71 @@ def syn_tvqa(seed=77, vfeat_dim=VFEAT_DIM):
     4 videos x 5 candidates, clips of 40-100 frames, QA strings of 20-60 tokens (joint rows of
     60-160 tokens, so some take the long-row attention path)."""
     return syn_videoqa_batch(n_videos=4, n_cand=5, seed=seed, vfeat_dim=vfeat_dim)
+
+
+def syn_violin_items(n_videos=4, n_statements=2, seed=77, t_range=(20, 100), s_range=(4, 20),
+                     l_range=(4, 40), q_range=(8, 40), vfeat_dim=VFEAT_DIM, vocab=50265):
+    """Dataset items of data/violin.py:63-115 (ViolinDataset.__getitem__), one per video: the clip
+    (make_clip), its `n_statements` statements as `[SEP] + ids` (`q_range` tokens with the [SEP])
+    and their targets. Two statements are a training pair, a statement and its opposite, so the
+    targets are {1, 0} in random order; one statement is an eval item (ViolinEvalDataset) with a
+    random target."""
+    gen = torch.Generator().manual_seed(seed)
+    rnd = random.Random(seed)
+    items = []
+    for _ in range(n_videos):
+        T = rnd.randint(*t_range)
+        S = min(rnd.randint(*s_range), T)
+        cuts = sorted(rnd.sample(range(1, T), S - 1)) if S > 1 else []
+        bounds = [0] + cuts + [T]
+        groups = [list(range(bounds[s], bounds[s + 1])) for s in range(len(bounds) - 1)]
+        clip = make_clip(gen, T, groups, [rnd.randint(*l_range) for _ in groups], vfeat_dim,
+                         vocab)
+        statements = [torch.cat([torch.tensor([SEP]),
+                                 torch.randint(3, vocab, (rnd.randint(*q_range) - 1,),
+                                               generator=gen)])
+                      for _ in range(n_statements)]
+        if n_statements == 2:
+            targets = rnd.sample([1, 0], 2)
+        else:
+            targets = [rnd.randrange(2) for _ in range(n_statements)]
+        items.append({"clip": clip, "statements": statements, "targets": targets})
+    return items
+
+
+def syn_violin_batch(n_videos=4, n_statements=2, seed=77, t_range=(20, 100), s_range=(4, 20),
+                     l_range=(4, 40), q_range=(8, 40), vfeat_dim=VFEAT_DIM, vocab=50265):
+    """data/violin.py:118-141 (violin_collate) over `syn_violin_items`: every (video, statement)
+    pair is one clip item of `video_collate` whose subtitles are each followed by the statement,
+    so the rows are video-major. `q_input_ids / q_pos_ids / q_attn_masks` hold the statements
+    (txt_input_collate: ids padded with 1, positions clamped at 511), `targets` (rows, 1) 1 for a
+    true statement and 0 for a false one."""
+    items = syn_violin_items(n_videos, n_statements, seed, t_range, s_range, l_range, q_range,
+                             vfeat_dim, vocab)
+    rows, stmts, targets = [], [], []
+    for it in items:
+        clip = it["clip"]
+        for st, t in zip(it["statements"], it["targets"]):
+            rows.append({"feats": clip["feats"], "sub2frames": clip["sub2frames"],
+                         "subs": [torch.cat([s, st]) for s in clip["subs"]]})
+            stmts.append(st)
+            targets.append(t)
+    b = video_batch(rows)
+    q = max(len(x) for x in stmts)
+    ids = torch.full((len(stmts), q), PAD, dtype=torch.long)
+    masks = torch.zeros(len(stmts), q, dtype=torch.long)
+    for i, x in enumerate(stmts):
+        ids[i, :len(x)] = x
+        masks[i, :len(x)] = 1
+    b["targets"] = torch.tensor(targets, dtype=torch.long).unsqueeze(1)
+    b["q_input_ids"], b["q_attn_masks"] = ids, masks
+    b["q_pos_ids"] = torch.arange(q, dtype=torch.long).clamp(max=511).unsqueeze(0)
+    return b
+
+
+def syn_violin(seed=77, vfeat_dim=VFEAT_DIM):
+    """VIOLIN-shaped training batch of one GPU (config/train-violin-8gpu.json: train_batch_size 4):
+    4 statement pairs = 8 rows, clips of 20-100 frames in 4-20 subtitles, statements of 8-40
+    tokens with the [SEP] (joint rows of 28-140 tokens, so some take the long-row attention
+    path)."""
+    return syn_violin_batch(n_videos=4, n_statements=2, seed=seed, vfeat_dim=vfeat_dim)

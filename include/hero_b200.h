@@ -511,7 +511,12 @@ int hero_temporal_nms(const float* score, const int32_t* mom, int32_t nq, int32_
  * The second softmax runs over the candidates (the reference's dim=1); masks may differ between
  * the candidates of a video. a and b (fp32 [Nv*Nq*L]) are written for the backward.
  * Bounds: 1 <= Nq <= 16, 1 <= L <= 512, H a positive multiple of 8, Nv >= 1; h, w_qa, w_st, the
- * pooled tensors, their gradients and dh 16-byte aligned. Two launches forward, four backward. */
+ * pooled tensors, their gradients and dh 16-byte aligned. Two launches forward, four backward.
+ * Single pooling (VIOLIN, model/violin.py:30-47): w_st == NULL computes only a and qa_pooled, the
+ * softmax over l; b and st_pooled must then be NULL too (in the backward also d_st_pooled and
+ * dw_st), and a mix of NULL and non-NULL is HERO_ERR_INVALID. The forward then launches only the
+ * Nv*Nq softmax-over-l blocks; the backward computes d a, the a.dq + ga.w_qa part of dh and one
+ * weight-gradient partial per chunk. The scratch size below serves both modes. */
 int hero_qa_pool_fwd(const float* h, const int32_t* map, const float* mask, const float* w_qa,
                      const float* w_st, int32_t Nv, int32_t Nq, int32_t L, int32_t H, float* a,
                      float* b, float* qa_pooled, float* st_pooled, void* stream);
