@@ -157,6 +157,7 @@ def _declare(lib):
     lib.hero_qa_pool_bwd_scratch_floats.argtypes = [i32, i32, i32, i32]
     sig("hero_qa_pool_bwd", vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp,
         vp)
+    sig("hero_dec_attn_fwd", vp, i64, vp, i64, vp, i64, vp, vp, i32, i32, i32, f32, vp, i64, vp)
 
 
 def lib():

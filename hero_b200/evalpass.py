@@ -824,6 +824,26 @@ def validate_violin(model, loader, split, save_logits=False):
     return val_log, results, logits
 
 
+def decode_tvc(model, loader, *, max_step, bos, eos, tokenizer):
+    """inf_tvc.py:83-98 / train_tvc.py:259-283 (decode / validate) for one process: greedy captions
+    of every segment of every batch (tvc.TvcGenerator, one device->host copy per batch) as
+    `{'vid_name', 'clip_id', 'ts', 'descs': [{'desc': caption}]}` records, in batch order. The
+    tokenizer is any object with `convert_ids_to_tokens` / `convert_tokens_to_string`. Gathering
+    across ranks (all_gather_list) and the COCO caption metrics are left to the caller."""
+    from .tvc import TvcGenerator
+    generator = TvcGenerator(model, max_step, bos, eos, fp16=False)
+    model.eval()
+    results = []
+    for batch in loader:
+        outputs = generator.greedy_decode(batch)
+        for vid, cid, ts, out_ids in zip(batch["vid_names"], batch["clip_ids"], batch["all_ts"],
+                                         outputs):
+            output = tokenizer.convert_tokens_to_string(tokenizer.convert_ids_to_tokens(out_ids))
+            results.append({"vid_name": vid, "clip_id": cid, "ts": ts,
+                            "descs": [{"desc": output}]})
+    return results
+
+
 class ModelSaver(object):
     """utils/save.py:112-130."""
 

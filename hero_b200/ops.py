@@ -692,3 +692,40 @@ def qa_pool_bwd(h, frame_map, mask, w_qa, w_st, a, b, d_qa, d_st, nv, nq, length
                                            _ptr(w_st), _ptr(a), _ptr(b), _ptr(d_qa), _ptr(d_st),
                                            nv, nq, length, H, _ptr(scratch), _ptr(dh),
                                            _ptr(dw_qa), _ptr(dw_st), _stream()))
+
+
+# ---------------------------------------------------------------------------------------------
+# TVC decoder attention (hero_b200/csrc/decode.cu)
+DEC_HEAD_DIM, DEC_MAX_KV = 64, 1024
+
+
+def _dec_attn_bounds(rows, heads, head_dim, max_kv_len, min_kv_len):
+    if rows < 0 or heads < 1 or head_dim != DEC_HEAD_DIM or not 1 <= min_kv_len <= max_kv_len \
+            or max_kv_len > DEC_MAX_KV:
+        raise ValueError(f"dec_attn_fwd: (rows, heads, head_dim, kv_len range) = ({rows}, {heads}, "
+                         f"{head_dim}, [{min_kv_len}, {max_kv_len}]); the kernel takes head_dim "
+                         f"{DEC_HEAD_DIM} and key ranges of 1 to {DEC_MAX_KV} rows")
+
+
+def dec_attn_fwd(q, k, v, kv_off, kv_len, out, *, heads, max_kv_len, min_kv_len=1,
+                 head_dim=DEC_HEAD_DIM):
+    """out[i] = softmax(q_i . K^T / sqrt(d)) V per head over the rows [kv_off[i], kv_off[i] +
+    kv_len[i]) of k / v (`hero_dec_attn_fwd`). q, k, v, out: bf16 2-D views with unit column
+    stride (their row strides are the leading dimensions: a view into a QKV cache works as is);
+    kv_off / kv_len: int32 [rows] on the device. `max_kv_len` / `min_kv_len` are the host-known
+    bounds of kv_len, checked here before the launch."""
+    rows = out.shape[0]
+    _dec_attn_bounds(rows, heads, head_dim, max_kv_len, min_kv_len)
+    _require_cuda(q, k, v, kv_off, kv_len, out)
+    for t in (q, k, v, out):
+        assert t.dtype == BF16 and t.dim() == 2 and t.stride(1) == 1
+        assert t.shape[1] >= heads * head_dim
+    assert q.shape[0] >= rows
+    for t in (kv_off, kv_len):
+        assert t.dtype == torch.int32 and t.is_contiguous() and t.numel() >= rows
+    _count()
+    _lib.check(_lib.lib().hero_dec_attn_fwd(_ptr(q), q.stride(0), _ptr(k), k.stride(0), _ptr(v),
+                                            v.stride(0), _ptr(kv_off), _ptr(kv_len), rows, heads,
+                                            head_dim, 1.0 / (head_dim ** 0.5), _ptr(out),
+                                            out.stride(0), _stream()))
+    return out

@@ -26,7 +26,9 @@ def _ordered_named_params(module):
     for name, p in named:
         if name in placed:
             continue
-        m = re.match(r"(.*attention\.self\.)query\.weight$", name)
+        # encoder layers, and the two attentions of the TVC decoder layers (model/tvc.py:107-116)
+        m = re.match(r"(.*(?:attention\.self|\.self_attention|\.dec_enc_attention)\.)query\.weight$",
+                     name)
         if m:
             base = m.group(1)
             group = [base + s for s in ("query.weight", "key.weight", "value.weight",

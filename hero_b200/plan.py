@@ -618,3 +618,78 @@ def qa_plan_inputs(batch, prefix="qa"):
 def qa_plan(batch, prefix="qa"):
     """QaPlan of a video_qa_collate batch (prefix "qa") or a violin_collate batch ("q")."""
     return QaPlan(**qa_plan_inputs(batch, prefix))
+
+
+class TvcPlan:
+    """Caption segments of a TVC batch (model/tvc.py:219-238, data/tvc.py:100-161): segment s of
+    the flattened `clip_ranges` is the frames [st, ed) of its video. Instead of padding the segments
+    to (n_seg, Lv, H), the plan lists the packed clip-level rows of every segment's frames
+    (CSR `seg_off` into `seg_src`); the decoder's cross-attention K / V are computed once per layer
+    over those gathered rows, and caption s attends to rows [kv_off[s], kv_off[s] + kv_len[s]).
+
+    An empty segment (st == ed == nframes when the caption starts past the last frame,
+    data/tvc.py:119-138) is all padding in the reference, masked uniformly, so its cross-attention
+    returns exactly the value bias. `seg_src` ends with one extra -1 entry, a zero input row whose
+    K / V are the biases; empty segments attend to it alone. A batch whose segments are all empty
+    raises ValueError. Built on the host from `clip_ranges` (a host tuple) and the ReprPlan: no
+    device read-back."""
+
+    def __init__(self, clip_ranges, rplan):
+        s = rplan.c.seq
+        segs = [(v, int(st), int(ed)) for v, rs in enumerate(clip_ranges) for st, ed in rs]
+        if len(clip_ranges) != s.rows:
+            raise ValueError(f"clip_ranges lists {len(clip_ranges)} videos, the batch has {s.rows}")
+        if not segs:
+            raise ValueError("the batch has no caption segment")
+        src, off, lens = [], [], []
+        n = 0
+        for v, st, ed in segs:
+            if not 0 <= st <= ed <= int(s.lens[v]):
+                raise ValueError(f"segment [{st}, {ed}) of video {v} is outside its "
+                                 f"{int(s.lens[v])} frames")
+            rows = s.pad_to_tok[v * s.length + np.arange(st, ed)]
+            if (rows < 0).any():
+                raise ValueError(f"segment [{st}, {ed}) of video {v} covers a masked frame")
+            src.append(rows)
+            off.append(n)
+            lens.append(ed - st)
+            n += ed - st
+        if n == 0:
+            raise ValueError("every caption segment of the batch is empty; the decoder needs at "
+                             "least one frame to attend to")
+        self.n_seg = len(segs)
+        self.n_rows = n + 1                                   # + the zero row of empty segments
+        self.seg_src = np.concatenate(src + [np.array([-1])]).astype(np.int32)
+        self.seg_off = np.concatenate([off, [n]]).astype(np.int32)
+        lens = np.asarray(lens, np.int32)
+        self.seg_len = lens
+        self.kv_off = np.where(lens > 0, self.seg_off[:-1], n).astype(np.int32)
+        self.kv_len = np.maximum(lens, 1).astype(np.int32)
+        self.max_kv = int(self.kv_len.max())
+        self.dev = None
+
+    def decode_arrays(self, max_step):
+        """Per-step index arrays of greedy decoding over a KV cache laid out [n_seg, max_step, *]:
+        `self_off` [n_seg] (first cache row of each caption), `step_len` [max_step, n_seg] (keys
+        0..t at step t), `step_pos` [max_step, n_seg] (position id t)."""
+        n, t = self.n_seg, np.arange(max_step, dtype=np.int32)
+        return {"self_off": (np.arange(n, dtype=np.int32) * max_step).astype(np.int32),
+                "step_len": np.repeat(t + 1, n).astype(np.int32),
+                "step_pos": np.repeat(t, n).astype(np.int32)}
+
+    def forced_arrays(self, length):
+        """Index arrays of a teacher-forced pass over (n_seg, length) caption rows, row-major:
+        causal self-attention ranges and each row's cross-attention range."""
+        n = self.n_seg
+        t = np.tile(np.arange(length, dtype=np.int32), n)
+        return {"tf_self_off": np.repeat(np.arange(n, dtype=np.int64) * length, length)
+                .astype(np.int32),
+                "tf_self_len": (t + 1).astype(np.int32),
+                "tf_kv_off": np.repeat(self.kv_off, length).astype(np.int32),
+                "tf_kv_len": np.repeat(self.kv_len, length).astype(np.int32)}
+
+    def to(self, device, extra=None, staging=None):
+        """Upload the segment maps and `extra` (decode_arrays / forced_arrays) in one copy."""
+        a = {"seg_src": self.seg_src, "kv_off": self.kv_off, "kv_len": self.kv_len}
+        a.update(extra or {})
+        return DeviceIndex(a, torch.device(device), staging)

@@ -379,3 +379,89 @@ def syn_violin(seed=77, vfeat_dim=VFEAT_DIM):
     tokens with the [SEP] (joint rows of 28-140 tokens, so some take the long-row attention
     path)."""
     return syn_violin_batch(n_videos=4, n_statements=2, seed=seed, vfeat_dim=vfeat_dim)
+
+
+# --------------------------------------------------------------------------------------------
+# TVC captioning (data/tvc.py). Ids of the RoBERTa vocabulary: <s> = 0, </s> = 2.
+BOS, EOS = CLS, SEP
+FRAME_INTERVAL = 1.5          # vfeat_interval of train-tvc-8gpu.json
+
+
+def syn_tvc_items(n_videos=8, seed=77, t_range=(20, 100), s_range=(4, 20), l_range=(4, 40),
+                  seg_range=(2, 6), c_range=(6, 24), n_empty=1, vfeat_dim=VFEAT_DIM, vocab=50265):
+    """Dataset items of data/tvc.py:100-114 / 170-190, one per video: the clip (make_clip), its
+    `seg_range` caption segments as (st, ed) frame ranges with their time stamps, and per segment a
+    caption of `c_range` tokens as input ids `[BOS] + cap` and targets `cap + [EOS]`. The last
+    segment of the first `n_empty` videos after the first starts past the last frame, so
+    get_st_ed_label gives st == ed == nframes (data/tvc.py:119-138): an empty segment."""
+    gen = torch.Generator().manual_seed(seed)
+    rnd = random.Random(seed)
+    items = []
+    for v in range(n_videos):
+        T = rnd.randint(*t_range)
+        S = min(rnd.randint(*s_range), T)
+        cuts = sorted(rnd.sample(range(1, T), S - 1)) if S > 1 else []
+        bounds = [0] + cuts + [T]
+        groups = [list(range(bounds[s], bounds[s + 1])) for s in range(len(bounds) - 1)]
+        clip = make_clip(gen, T, groups, [rnd.randint(*l_range) for _ in groups], vfeat_dim,
+                         vocab)
+        ranges, ts, caps = [], [], []
+        for k in range(rnd.randint(*seg_range)):
+            if 1 <= v <= n_empty and k == 0:
+                st = ed = T
+            else:
+                st = rnd.randrange(T)
+                ed = min(T, st + rnd.randint(1, 16))
+            ranges.append((st, ed))
+            ts.append([st * FRAME_INTERVAL, max(ed, st + 1) * FRAME_INTERVAL])
+            caps.append(torch.randint(3, vocab, (rnd.randint(*c_range),), generator=gen))
+        if 1 <= v <= n_empty:           # the empty segment last, as a late caption would be
+            ranges, ts, caps = ranges[1:] + ranges[:1], ts[1:] + ts[:1], caps[1:] + caps[:1]
+        items.append({"clip": clip, "vid": f"v{v}", "clip_ranges": ranges, "ts": ts,
+                      "clip_ids": [1000 * v + k for k in range(len(ranges))],
+                      "input_ids": [torch.cat([torch.tensor([BOS]), c]) for c in caps],
+                      "tgt_ids": [torch.cat([c, torch.tensor([EOS])]) for c in caps]})
+    return items
+
+
+def syn_tvc_batch(n_videos=8, seed=77, t_range=(20, 100), s_range=(4, 20), l_range=(4, 40),
+                  seg_range=(2, 6), c_range=(6, 24), n_empty=1, vfeat_dim=VFEAT_DIM, vocab=50265,
+                  split="train"):
+    """TvcTrainDataset.collate (split "train", data/tvc.py:140-161) or TvcValDataset.collate
+    ("val", :192-218) over `syn_tvc_items`: `cap_attn_mask` (one 1 per segment frame, padded with
+    0), `clip_ranges` (a tuple per video), the video_collate keys, and for training the captions
+    (`cap_input_ids` padded with 1, `cap_pos_ids`, `cap_tgt_ids` padded with -1); for validation
+    the metadata `vid_names / clip_ids / all_ts / gts`."""
+    items = syn_tvc_items(n_videos, seed, t_range, s_range, l_range, seg_range, c_range, n_empty,
+                          vfeat_dim, vocab)
+    ranges = [r for it in items for r in it["clip_ranges"]]
+    n_seg, max_l = len(ranges), max(ed - st for st, ed in ranges)
+    mask = torch.zeros(n_seg, max_l, dtype=torch.long)
+    for i, (st, ed) in enumerate(ranges):
+        mask[i, :ed - st] = 1
+    b = {"cap_attn_mask": mask,
+         "clip_ranges": tuple(tuple(it["clip_ranges"]) for it in items)}
+    if split == "train":
+        ins = [x for it in items for x in it["input_ids"]]
+        tgts = [x for it in items for x in it["tgt_ids"]]
+        lt = max(len(x) for x in ins)
+        ids = torch.full((n_seg, lt), PAD, dtype=torch.long)
+        tgt = torch.full((n_seg, lt), -1, dtype=torch.long)
+        for i, (x, y) in enumerate(zip(ins, tgts)):
+            ids[i, :len(x)] = x
+            tgt[i, :len(y)] = y
+        b.update({"cap_input_ids": ids, "cap_pos_ids": torch.arange(lt).unsqueeze(0),
+                  "cap_tgt_ids": tgt})
+    b.update(video_batch([it["clip"] for it in items]))
+    if split != "train":
+        b["vid_names"] = [it["vid"] for it in items for _ in it["clip_ranges"]]
+        b["clip_ids"] = [c for it in items for c in it["clip_ids"]]
+        b["all_ts"] = [t for it in items for t in it["ts"]]
+        b["gts"] = [f"caption {c}" for c in b["clip_ids"]]
+    return b
+
+
+def syn_tvc_val(seed=77, vfeat_dim=VFEAT_DIM):
+    """TVC validation batch of val_batch_size 8 (train-tvc-8gpu.json): 8 videos of ragged clips,
+    2-6 caption segments each, one of them empty."""
+    return syn_tvc_batch(n_videos=8, seed=seed, vfeat_dim=vfeat_dim, split="val")

@@ -1,0 +1,360 @@
+"""HeroForTvc and TvcGenerator (model/tvc.py): TVC video captioning, inference.
+
+The encoder is HERO's ('repr'); each caption segment is a frame range of its video's clip-level
+output. The decoder is a 2-layer transformer with causal self-attention and cross-attention to the
+segment frames, its word embedding and LM head tied to the cross-modal encoder's. On this path:
+
+    ReprPlan + TvcPlan (host)  ->  repr_packed  ->  gather the segment rows (+ one zero row)  ->
+    per decoder layer: cross K / V of all segment frames, one GEMM
+    per position: word[id] + pos[t] -> LayerNorm (ln_fwd) -> per layer: QKV GEMM, dec_attn_fwd
+      (causal range), dense + residual -> LayerNorm, Q GEMM, dec_attn_fwd (segment range),
+      dense + residual -> LayerNorm, FFN (GELU) -> dense + residual -> LayerNorm  ->
+    LM-head transform (GEMM + GELU, LayerNorm) -> vocabulary GEMM (fp32 logits)
+
+`forward` runs that over every position of the teacher-forced captions at once. Greedy decoding
+runs it one position at a time against a KV cache that the QKV GEMM writes straight into, and takes
+the argmax with `rank_topk(k=1)` into the next step's id buffer: the reference instead re-runs the
+decoder and the full-vocabulary logits over the whole prefix at every step (model/tvc.py:301-330).
+
+Inference only. Decoder training (its attention backward and the label-smoothed loss gradient) is
+not on the CUDA path yet: `forward` raises NotImplementedError in training mode or when it would
+have to build an autograd graph.
+"""
+import math
+from collections import defaultdict
+
+import numpy as np
+import torch
+from torch import nn
+
+from . import ops
+from .layers import BertIntermediate, BertLayerNorm, BertOutput, BertSelfAttention, BertSelfOutput
+from .model import HeroModel
+from .params import flat_of
+from .plan import PLAN_KEY, ReprPlan, TvcPlan
+
+BF16 = torch.bfloat16
+MAX_DECODE_STEP = 1023      # position table of 1024 entries (hero_tvc.json d_config)
+
+
+class LabelSmoothingLoss(nn.Module):
+    """Parameter container of model/tvc.py:19-64 (its `one_hot` buffer is part of the reference's
+    state_dict). The loss itself is computed from the fused LM-head cross entropy in
+    `HeroForTvc._loss`."""
+
+    def __init__(self, label_smoothing, tgt_vocab_size, ignore_index=-100, reduction="none"):
+        assert 0.0 < label_smoothing <= 1.0
+        super().__init__()
+        self.ignore_index = ignore_index
+        self.smoothing_value = label_smoothing / (tgt_vocab_size - 1)
+        self.register_buffer("one_hot", torch.full((tgt_vocab_size,),
+                                                   self.smoothing_value).unsqueeze(0))
+        self.confidence = 1.0 - label_smoothing
+        self.reduction = reduction
+
+
+class BertDecoderLayer(nn.Module):
+    """model/tvc.py:107-154 (parameter names kept, `intermidiate` included)."""
+
+    def __init__(self, config):
+        super().__init__()
+        self.config = config
+        self.self_attention = BertSelfAttention(config)
+        self.add_norm_1 = BertSelfOutput(config)
+        self.dec_enc_attention = BertSelfAttention(config)
+        self.add_norm_2 = BertSelfOutput(config)
+        self.intermidiate = BertIntermediate(config)
+        self.add_norm_3 = BertOutput(config)
+
+    def weights(self, flat):
+        """bf16 GEMM operands and fp32 biases / LayerNorm parameters of the layer; q / k / v of
+        both attentions are adjacent in the flat buffer (params._ordered_named_params)."""
+        sa, ca = self.self_attention, self.dec_enc_attention
+        H = sa.query.weight.shape[1]
+        for a, b in ((sa.query, sa.key), (sa.key, sa.value), (ca.key, ca.value)):
+            if not (flat.contiguous_after(a.weight, b.weight) and
+                    flat.contiguous_after(a.bias, b.bias)):
+                raise RuntimeError("decoder query/key/value parameters are not adjacent in the "
+                                   "flat buffer")
+        n1, n2, n3 = self.add_norm_1, self.add_norm_2, self.add_norm_3
+        return {
+            "wqkv": flat.bf16_span(sa.query.weight, 3 * H * H, (3 * H, H)),
+            "bqkv": flat.f32_span(sa.query.bias, 3 * H, (3 * H,)),
+            "wo1": flat.bf16(n1.dense.weight), "bo1": n1.dense.bias.detach(), "ln1": n1.LayerNorm,
+            "wq_c": flat.bf16(ca.query.weight), "bq_c": ca.query.bias.detach(),
+            "wkv_c": flat.bf16_span(ca.key.weight, 2 * H * H, (2 * H, H)),
+            "bkv_c": flat.f32_span(ca.key.bias, 2 * H, (2 * H,)),
+            "wo2": flat.bf16(n2.dense.weight), "bo2": n2.dense.bias.detach(), "ln2": n2.LayerNorm,
+            "w1": flat.bf16(self.intermidiate.dense.weight),
+            "b1": self.intermidiate.dense.bias.detach(),
+            "w2": flat.bf16(n3.dense.weight), "b2": n3.dense.bias.detach(), "ln3": n3.LayerNorm,
+        }
+
+
+class BertDecoder(nn.Module):
+    """model/tvc.py:157-193: the layers and the persistent causal-mask buffer of the reference
+    (kept for its state_dict; the kernels take key ranges instead)."""
+
+    def __init__(self, config):
+        super().__init__()
+        self.num_heads = config.num_attention_heads
+        self.layer = nn.ModuleList([BertDecoderLayer(config)
+                                    for _ in range(config.num_hidden_layers)])
+        tri_mask = torch.tril(torch.ones(1024, 1024), diagonal=0)
+        tri_mask = (1.0 - tri_mask) * -10000.0
+        self.register_buffer("tri_mask", tri_mask)
+
+
+def _ln(x, ln, y, n_rows, y_f32=None, **kw):
+    ops.ln_fwd(x, ln.weight.detach(), ln.bias.detach(), ln.eps, y, n_rows=n_rows, y_f32=y_f32,
+               **kw)
+
+
+class _Workspace:
+    """Activation buffers of one decoder pass over m rows (reused by every layer / step)."""
+
+    def __init__(self, m, H, inter, V, device):
+        f32 = torch.float32
+        self.x, self.a, self.b = (torch.empty(m, H, dtype=BF16, device=device) for _ in range(3))
+        self.x32, self.a32, self.b32 = (torch.empty(m, H, dtype=f32, device=device)
+                                        for _ in range(3))
+        self.s = torch.empty(m, H, dtype=f32, device=device)
+        self.ctx = torch.empty(m, H, dtype=BF16, device=device)
+        self.qc = torch.empty(m, H, dtype=BF16, device=device)
+        self.f = torch.empty(m, inter, dtype=BF16, device=device)
+        self.t = torch.empty(m, H, dtype=BF16, device=device)
+        self.h = torch.empty(m, H, dtype=BF16, device=device)
+        self.logits = torch.empty(m, V, dtype=f32, device=device)
+
+
+class HeroForTvc(HeroModel):
+    def __init__(self, config, vfeat_dim, max_frm_seq_len, lsr=0.1):
+        super().__init__(config, vfeat_dim, max_frm_seq_len)
+        self.config = config
+        d = config.d_config
+        self.position_embeddings = nn.Embedding(d.max_position_embeddings, d.hidden_size)
+        self.emb_LayerNorm = BertLayerNorm(d.hidden_size, eps=1e-5)
+        self.decoder = BertDecoder(d)
+        self.lsr = lsr
+        if lsr > 0:
+            self.loss_func = LabelSmoothingLoss(lsr, config.f_config.vocab_size, ignore_index=-1,
+                                                reduction="none")
+        else:
+            self.loss_func = nn.CrossEntropyLoss(ignore_index=-1, reduction="none")
+        self.v_encoder.initialize()
+
+    # ------------------------------------------------------------------ encoder side
+    def encode(self, batch):
+        """model/tvc.py:219-238 without the padding: (packed clip-level outputs fp32
+        [n_c_tokens, H] of HierarchicalVlModel.repr_packed, TvcPlan of the caption segments). Uses
+        the ReprPlan attached with plan.attach_plan, else builds it (one device->host read of the
+        masks)."""
+        if not isinstance(batch, defaultdict):
+            batch = defaultdict(lambda: None, batch)
+        rplan = batch[PLAN_KEY]
+        if rplan is None:
+            rplan = ReprPlan(batch)
+        tplan = TvcPlan(batch["clip_ranges"], rplan)
+        flat_of(self, batch["c_v_feats"].device)   # one flat buffer for encoder and decoder
+        y, _ = self.v_encoder.repr_packed(batch, rplan)
+        return y, tplan
+
+    def _gather_segments(self, y, tplan, tdev):
+        rows = torch.empty(tplan.n_rows, y.shape[1], dtype=y.dtype, device=y.device)
+        ops.gather_rows(y.contiguous(), tdev.seg_src, rows)
+        if rows.dtype == BF16:
+            return rows
+        return ops.cast_bf16(rows, torch.empty(rows.shape, dtype=BF16, device=y.device))
+
+    def _weights(self, device):
+        flat = flat_of(self, device)
+        fe = self.v_encoder.f_encoder
+        head = fe.lm_head
+        emb = fe.embeddings.word_embeddings.weight
+        return flat, {
+            "layers": [l.weights(flat) for l in self.decoder.layer],
+            "word": emb.detach(), "pos": self.position_embeddings.weight.detach(),
+            "emb_bf16": flat.bf16(emb), "lm_bias": head.bias.detach(),
+            "dense": flat.bf16(head.dense.weight), "dense_b": head.dense.bias.detach(),
+            "n_valid": emb.shape[0] - fe.vocab_pad}
+
+    def _cross_kv(self, w, enc):
+        """Cross-attention K | V [rows + 1, 2H] of every decoder layer, one GEMM each."""
+        out = []
+        for lw in w["layers"]:
+            kv = torch.empty(enc.shape[0], lw["wkv_c"].shape[0], dtype=BF16, device=enc.device)
+            out.append(ops.gemm(enc, lw["wkv_c"], kv, bias=lw["bkv_c"]))
+        return out
+
+    def _check_inference(self):
+        if self.training or (torch.is_grad_enabled() and
+                             any(p.requires_grad for p in self.parameters())):
+            raise NotImplementedError(
+                "TVC decoder training is not on the CUDA path yet: HeroForTvc runs inference "
+                "only. Call it in eval mode under torch.no_grad().")
+
+    # ------------------------------------------------------------------ decoder
+    def _positions(self, w, ws, ids, pos, n_rows, layers, self_qkv, self_rng, cross_kv, cross_rng):
+        """One decoder pass over n_rows positions: embedding, every layer, LM-head transform and
+        the vocabulary logits (into ws.logits). `self_qkv(l)` -> (QKV output view, K view, V view)
+        of layer l; `self_rng` / `cross_rng` = (kv_off, kv_len, max_len)."""
+        H = ws.x.shape[1]
+        heads = self.decoder.num_heads
+        _ln(w["word"], self.emb_LayerNorm, ws.x, n_rows, y_f32=ws.x32, x_rows=ids,
+            add_tab=w["pos"], add_idx=pos)
+        for l, lw in enumerate(layers):
+            qkv, k, v = self_qkv(l)
+            ops.gemm(ws.x, lw["wqkv"], qkv, bias=lw["bqkv"])
+            ops.dec_attn_fwd(qkv[:, :H], k, v, self_rng[0], self_rng[1], ws.ctx, heads=heads,
+                             max_kv_len=self_rng[2])
+            ops.gemm(ws.ctx, lw["wo1"], ws.s, bias=lw["bo1"], resid=ws.x32)
+            _ln(ws.s, lw["ln1"], ws.a, n_rows, y_f32=ws.a32)
+            ops.gemm(ws.a, lw["wq_c"], ws.qc, bias=lw["bq_c"])
+            kv = cross_kv[l]
+            ops.dec_attn_fwd(ws.qc, kv[:, :H], kv[:, H:], cross_rng[0], cross_rng[1], ws.ctx,
+                             heads=heads, max_kv_len=cross_rng[2])
+            ops.gemm(ws.ctx, lw["wo2"], ws.s, bias=lw["bo2"], resid=ws.a32)
+            _ln(ws.s, lw["ln2"], ws.b, n_rows, y_f32=ws.b32)
+            ops.gemm(ws.b, lw["w1"], ws.f, bias=lw["b1"], act=ops.ACT_GELU)
+            ops.gemm(ws.f, lw["w2"], ws.s, bias=lw["b2"], resid=ws.b32)
+            _ln(ws.s, lw["ln3"], ws.x, n_rows, y_f32=ws.x32)
+        head = self.v_encoder.f_encoder.lm_head
+        ops.gemm(ws.x, w["dense"], ws.t, bias=w["dense_b"], act=ops.ACT_GELU)
+        _ln(ws.t, head.LayerNorm, ws.h, n_rows)
+        ops.gemm(ws.h, w["emb_bf16"], ws.logits, bias=w["lm_bias"])
+
+    def _workspace(self, m, device):
+        d = self.config.d_config
+        V = self.v_encoder.f_encoder.embeddings.word_embeddings.weight.shape[0]
+        return _Workspace(m, d.hidden_size, d.intermediate_size, V, device)
+
+    def forward(self, batch, mode="train", compute_loss=True):
+        """model/tvc.py:268-276. Without `compute_loss`: the teacher-forced logits (N, Lt, V) fp32,
+        every position computed (padded ones included). With it: the reference's per-token loss,
+        LabelSmoothingLoss over the positions whose target is not -1 (lsr > 0), or cross entropy
+        with ignore_index -1 over all N * Lt positions (lsr == 0)."""
+        self._check_inference()
+        ids = batch["cap_input_ids"]
+        N, Lt = ids.shape
+        if Lt > self.position_embeddings.num_embeddings:
+            raise ValueError(f"captions of {Lt} tokens exceed the position table")
+        y, tplan = self.encode(batch)
+        device = y.device
+        if tplan.n_seg != N:
+            raise ValueError(f"{N} captions but {tplan.n_seg} segments in clip_ranges")
+        tdev = tplan.to(device, tplan.forced_arrays(Lt))
+        enc = self._gather_segments(y, tplan, tdev)
+        flat, w = self._weights(device)
+        cross = self._cross_kv(w, enc)
+        M = N * Lt
+        ws = self._workspace(M, device)
+        H = ws.x.shape[1]
+        qkv = torch.empty(M, 3 * H, dtype=BF16, device=device)
+        pos = batch["cap_pos_ids"].to(device=device)
+        pos = pos.expand(N, Lt).reshape(-1).to(torch.int32)
+        self._positions(w, ws, ids.to(device=device).reshape(-1).to(torch.int32), pos, M,
+                        w["layers"], lambda l: (qkv, qkv[:, H:2 * H], qkv[:, 2 * H:]),
+                        (tdev.tf_self_off, tdev.tf_self_len, Lt),
+                        cross, (tdev.tf_kv_off, tdev.tf_kv_len, tplan.max_kv))
+        n_valid = w["n_valid"]
+        if not compute_loss:
+            return ws.logits[:, :n_valid].view(N, Lt, n_valid)
+        return self._loss(ws, w, batch["cap_tgt_ids"], n_valid)
+
+    def _loss(self, ws, w, tgt, V):
+        device = ws.h.device
+        labels = tgt.reshape(-1).to(device)
+        valid = labels != -1
+        lab32 = torch.where(valid, labels, torch.zeros_like(labels)).to(torch.int32)
+        ce, lse = ops.lm_head_ce_fwd(ws.h, w["emb_bf16"], w["lm_bias"], lab32, V)
+        if self.lsr <= 0:
+            return torch.where(valid, ce, torch.zeros_like(ce))
+        # KL(q || softmax(z)) summed over the V columns, q = conf at the target, s elsewhere:
+        #   sum q log q - conf (z_t - lse) - s (sum_j z_j - z_t - (V - 1) lse)
+        # with z_t = lse - ce and sum_j z_j = h . sum_j E_j + sum_j b_j (one mat-vec against the
+        # column sum of the tied table)
+        lf = self.loss_func
+        conf, s = lf.confidence, lf.smoothing_value
+        esum = torch.zeros(ws.h.shape[1], dtype=torch.float32, device=device)
+        ops.colsum(w["emb_bf16"][:V], esum)
+        e8 = torch.zeros(8, ws.h.shape[1], dtype=BF16, device=device)
+        ops.cast_bf16(esum, e8[0])
+        zs8 = torch.empty(ws.h.shape[0], 8, dtype=torch.float32, device=device)
+        ops.gemm(ws.h, e8, zs8)
+        zsum = zs8[:, 0] + w["lm_bias"][:V].sum()
+        zt = lse - ce
+        ent = conf * math.log(conf) + (V - 1) * s * math.log(s)
+        loss = ent - conf * (zt - lse) - s * (zsum - zt - (V - 1) * lse)
+        if tgt.device.type == "cpu":
+            keep = torch.from_numpy(np.flatnonzero(tgt.reshape(-1).numpy() != -1)).to(device)
+            return loss[keep]
+        return loss[valid]
+
+
+class TvcGenerator(object):
+    """model/tvc.py:293-338 with the reference's constructor. `fp16` is accepted and ignored: the
+    path runs in bf16. `greedy_decode(batch)` returns, per caption, the greedy ids cut at the first
+    EOS, like the reference; it runs a fixed `max_step` positions (no early stop) with a KV cache
+    and returns the token chosen at each step, where the reference re-derives every position
+    from its last full pass (equal under causal masking)."""
+
+    def __init__(self, model, max_step, bos, eos, fp16):
+        self.model = model
+        self.max_step = max_step
+        self.bos = bos
+        self.eos = eos
+        self.fp16 = fp16
+
+    @torch.no_grad()
+    def greedy_decode(self, batch):
+        ids = self.decode_ids(batch)
+        return [self.cut_eos(row) for row in ids.tolist()]
+
+    @torch.no_grad()
+    def decode_ids(self, batch):
+        """Greedy ids (n_captions, max_step) as a host int32 tensor. Every upload of the batch
+        happens before the loop; the ids come back in one device->host copy."""
+        model, T = self.model, int(self.max_step)
+        if not 1 <= T <= MAX_DECODE_STEP:
+            raise ValueError(f"max_step = {T}: greedy decoding takes 1 to {MAX_DECODE_STEP} steps "
+                             f"(position table of {MAX_DECODE_STEP + 1})")
+        model._check_inference()
+        y, tplan = model.encode(batch)
+        device = y.device
+        N = tplan.n_seg
+        tdev = tplan.to(device, tplan.decode_arrays(T))
+        enc = model._gather_segments(y, tplan, tdev)
+        flat, w = model._weights(device)
+        cross = model._cross_kv(w, enc)
+        ws = model._workspace(N, device)
+        H = ws.x.shape[1]
+        caches = [torch.empty(N, T, 3 * H, dtype=BF16, device=device) for _ in w["layers"]]
+        rows = [c.view(N * T, 3 * H) for c in caches]
+        out = torch.empty(T + 1, N, dtype=torch.int32, device=device)
+        out[0].fill_(int(self.bos))
+        vals = torch.empty(N, 1, dtype=torch.float32, device=device)
+        n_valid = w["n_valid"]
+        for t in range(T):
+            step = slice(t * N, (t + 1) * N)
+            model._positions(w, ws, out[t], tdev.step_pos[step], N, w["layers"],
+                             lambda l: (caches[l][:, t], rows[l][:, H:2 * H], rows[l][:, 2 * H:]),
+                             (tdev.self_off, tdev.step_len[step], t + 1),
+                             cross, (tdev.kv_off, tdev.kv_len, tplan.max_kv))
+            ops.rank_topk(ws.logits, n_valid, 1, vals, out[t + 1].view(N, 1))
+        if device.type != "cuda":
+            return out[1:].t().clone()
+        # a non-blocking copy into pinned memory and an event wait: one copy, no stream sync
+        host = torch.empty((T, N), dtype=torch.int32, pin_memory=True)
+        host.copy_(out[1:], non_blocking=True)
+        done = torch.cuda.Event()
+        done.record()
+        done.synchronize()
+        return host.t()
+
+    def cut_eos(self, ids):
+        out_ids = []
+        for i in ids:
+            if i == self.eos:
+                break
+            out_ids.append(i)
+        return out_ids

@@ -533,6 +533,21 @@ int hero_qa_pool_bwd(const float* h, const int32_t* map, const float* mask, cons
                      const float* d_st_pooled, int32_t Nv, int32_t Nq, int32_t L, int32_t H,
                      float* scratch, float* dh, float* dw_qa, float* dw_st, void* stream);
 
+/* ---- TVC decoder attention (hero_b200/csrc/decode.cu) ----
+ * model/tvc.py:67-154 (BertDecEncAttention and the masked BertSelfAttention of BertDecoderLayer),
+ * forward only. For query row i < rows and head h, with q_i, k_j, v_j the 64 columns of head h of
+ * row i of q [*, ldq] and rows j of k [*, ldk], v [*, ldv] (bf16):
+ *   out[i, h] = sum_j softmax_j(q_i . k_j * scale) v_j   over j in [kv_off[i], kv_off[i] + kv_len[i])
+ * in fp32, stored as bf16 into out [rows, ldo]. A key range stands for the reference's -10000
+ * additive masks, whose weights are exactly zero in fp32. Causal self-attention, one greedy decode
+ * step against a KV cache, and cross-attention to a caption's segment frames differ only in the
+ * ranges. Bounds: head_dim == 64, 1 <= kv_len[i] <= 1024 (a row outside them is written as NaN),
+ * leading dimensions >= heads * 64, K rows 16-byte aligned, V rows 4-byte aligned. One launch. */
+int hero_dec_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
+                      int64_t ldv, const int32_t* kv_off, const int32_t* kv_len, int32_t rows,
+                      int32_t heads, int32_t head_dim, float scale, void* out, int64_t ldo,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif
