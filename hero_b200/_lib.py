@@ -102,6 +102,15 @@ class StackArgs(C.Structure):
     ]
 
 
+ADAMW_MAX_GROUPS = 8   # HERO_ADAMW_MAX_GROUPS
+
+
+class AdamwGroups(C.Structure):
+    """Mirror of `hero_adamw_groups`."""
+    _fields_ = [("n_groups", C.c_int32), ("step_size", C.c_float * ADAMW_MAX_GROUPS),
+                ("lr_wd", C.c_float * ADAMW_MAX_GROUPS)]
+
+
 def _declare(lib):
     vp, i32, i64, f32, u32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_uint32
     lib.hero_last_error.restype = C.c_char_p
@@ -140,6 +149,9 @@ def _declare(lib):
     sig("hero_relu_bwd_bf16", vp, vp, vp, i64, vp)
     sig("hero_adamw_step", vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, f32, vp, f32, vp)
     sig("hero_sumsq_f32", vp, i64, vp, vp)
+    sig("hero_adamw_step_groups", vp, vp, vp, vp, vp, i64, vp, vp, i32, C.POINTER(AdamwGroups),
+        f32, f32, f32, f32, vp, f32, vp)
+    sig("hero_sumsq_segments_f32", vp, i64, vp, vp, i32, i32, vp, vp)
     sig("hero_ce_finish", vp, i64, i32, vp, i32, vp, vp, vp)
     sig("hero_reduce_slots_f32", vp, vp, i32, i64, i64, f32, i32, vp)
     sig("hero_l2norm_split_f32", vp, i64, i32, f32, vp, vp, vp, vp)

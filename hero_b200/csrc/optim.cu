@@ -7,9 +7,41 @@
 
 namespace hero {
 
-// 16-byte vector accesses on all seven streams (p, g, m, v read; p, m, v + bf16 written: 30 B per
-// parameter). `clip` (device scalar: sum of squares of ALL gradients) folds global-norm clipping
-// into the update without a host round trip.
+// The AdamW update of the four consecutive elements [4i, 4i + 4): 16-byte vector accesses on all
+// seven streams (p, g, m, v read; p, m, v + bf16 written: 30 B per parameter). Shared by the
+// single-range and the segment-table kernels, so both compute bitwise the same values.
+__device__ __forceinline__ void adamw_vec4(float* __restrict__ p, const float* __restrict__ g,
+                                           float* __restrict__ m, float* __restrict__ v,
+                                           __nv_bfloat16* __restrict__ p_bf16, long long i,
+                                           float step_size, float beta1, float beta2, float ob1,
+                                           float ob2, float eps, float lr_wd, float grad_scale) {
+  const float4 g4 = __ldg(reinterpret_cast<const float4*>(g) + i);
+  float4 m4 = reinterpret_cast<float4*>(m)[i];
+  float4 v4 = reinterpret_cast<float4*>(v)[i];
+  float4 p4 = reinterpret_cast<float4*>(p)[i];
+  const float gr[4] = {g4.x * grad_scale, g4.y * grad_scale, g4.z * grad_scale, g4.w * grad_scale};
+  float mm[4] = {m4.x, m4.y, m4.z, m4.w}, vv[4] = {v4.x, v4.y, v4.z, v4.w};
+  float pp[4] = {p4.x, p4.y, p4.z, p4.w};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    mm[j] = beta1 * mm[j] + ob1 * gr[j];
+    vv[j] = beta2 * vv[j] + ob2 * gr[j] * gr[j];
+    pp[j] = pp[j] - step_size * (mm[j] / (sqrtf(vv[j]) + eps));
+    if (lr_wd > 0.0f) pp[j] = pp[j] - lr_wd * pp[j];
+  }
+  reinterpret_cast<float4*>(m)[i] = make_float4(mm[0], mm[1], mm[2], mm[3]);
+  reinterpret_cast<float4*>(v)[i] = make_float4(vv[0], vv[1], vv[2], vv[3]);
+  reinterpret_cast<float4*>(p)[i] = make_float4(pp[0], pp[1], pp[2], pp[3]);
+  if (p_bf16 != nullptr) {
+    uint2 u;
+    u.x = pack_bf16x2(pp[0], pp[1]);
+    u.y = pack_bf16x2(pp[2], pp[3]);
+    reinterpret_cast<uint2*>(p_bf16)[i] = u;
+  }
+}
+
+// `clip` (device scalar: sum of squares of ALL gradients) folds global-norm clipping into the
+// update without a host round trip.
 __global__ void __launch_bounds__(256)
 adamw_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
              float* __restrict__ v, __nv_bfloat16* __restrict__ p_bf16, long long n, float step_size,
@@ -22,31 +54,8 @@ adamw_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restri
   const long long n4 = n >> 2;
   const long long stride = (long long)gridDim.x * blockDim.x;
   const float ob1 = 1.0f - beta1, ob2 = 1.0f - beta2;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
-    const float4 g4 = __ldg(reinterpret_cast<const float4*>(g) + i);
-    float4 m4 = reinterpret_cast<float4*>(m)[i];
-    float4 v4 = reinterpret_cast<float4*>(v)[i];
-    float4 p4 = reinterpret_cast<float4*>(p)[i];
-    const float gr[4] = {g4.x * grad_scale, g4.y * grad_scale, g4.z * grad_scale, g4.w * grad_scale};
-    float mm[4] = {m4.x, m4.y, m4.z, m4.w}, vv[4] = {v4.x, v4.y, v4.z, v4.w};
-    float pp[4] = {p4.x, p4.y, p4.z, p4.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      mm[j] = beta1 * mm[j] + ob1 * gr[j];
-      vv[j] = beta2 * vv[j] + ob2 * gr[j] * gr[j];
-      pp[j] = pp[j] - step_size * (mm[j] / (sqrtf(vv[j]) + eps));
-      if (lr_wd > 0.0f) pp[j] = pp[j] - lr_wd * pp[j];
-    }
-    reinterpret_cast<float4*>(m)[i] = make_float4(mm[0], mm[1], mm[2], mm[3]);
-    reinterpret_cast<float4*>(v)[i] = make_float4(vv[0], vv[1], vv[2], vv[3]);
-    reinterpret_cast<float4*>(p)[i] = make_float4(pp[0], pp[1], pp[2], pp[3]);
-    if (p_bf16 != nullptr) {
-      uint2 u;
-      u.x = pack_bf16x2(pp[0], pp[1]);
-      u.y = pack_bf16x2(pp[2], pp[3]);
-      reinterpret_cast<uint2*>(p_bf16)[i] = u;
-    }
-  }
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride)
+    adamw_vec4(p, g, m, v, p_bf16, i, step_size, beta1, beta2, ob1, ob2, eps, lr_wd, grad_scale);
   // tail (n not a multiple of 4)
   for (long long i = (n4 << 2) + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
     const float gr = g[i] * grad_scale;
@@ -58,6 +67,20 @@ adamw_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restri
     v[i] = vi;
     p[i] = pi;
     if (p_bf16 != nullptr) p_bf16[i] = __float2bfloat16(pi);
+  }
+}
+
+// out[0] += sum of `s` over the 256 threads of the block (one atomic per block).
+__device__ __forceinline__ void block_sum_atomic_add(float s, float* __restrict__ out) {
+  s = warp_sum(s);
+  __shared__ float sm[8];
+  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x < 8) {
+    float t = sm[threadIdx.x];
+#pragma unroll
+    for (int o = 4; o > 0; o >>= 1) t += __shfl_xor_sync(0xffu, t, o);
+    if (threadIdx.x == 0) atomicAdd(out, t);
   }
 }
 
@@ -74,16 +97,63 @@ sumsq_kernel(const float* __restrict__ x, long long n, float* __restrict__ out) 
     const float t = x[i];
     s = fmaf(t, t, s);
   }
-  s = warp_sum(s);
-  __shared__ float sm[8];
-  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = s;
-  __syncthreads();
-  if (threadIdx.x < 8) {
-    float t = sm[threadIdx.x];
-#pragma unroll
-    for (int o = 4; o > 0; o >>= 1) t += __shfl_xor_sync(0xffu, t, o);
-    if (threadIdx.x == 0) atomicAdd(out, t);
+  block_sum_atomic_add(s, out);
+}
+
+// ---- segment tables: any set of disjoint ranges of the flat buffer, each in one of at most
+// HERO_ADAMW_MAX_GROUPS groups. A table is int64 triples (start, length, group), starts and lengths
+// multiples of 4 (checked on the host). Work is one grid-stride loop over the float4 index of the
+// concatenated segments, so it is spread over the threads as if the segments were one range. A
+// thread walks the table once; inside a segment its loop is the plain strided loop of adamw_kernel
+// (no per-iteration lookup). Elements outside every segment are never touched.
+struct AdamwGroupArgs {
+  float step_size[HERO_ADAMW_MAX_GROUPS];
+  float lr_wd[HERO_ADAMW_MAX_GROUPS];
+};
+
+__global__ void __launch_bounds__(256)
+adamw_groups_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
+                    float* __restrict__ v, __nv_bfloat16* __restrict__ p_bf16,
+                    const long long* __restrict__ seg, int n_seg, const AdamwGroupArgs groups,
+                    float beta1, float beta2, float eps, float grad_scale,
+                    const float* __restrict__ clip, float clip_max_norm) {
+  if (clip != nullptr) {
+    const float norm = sqrtf(__ldg(clip));
+    grad_scale *= fminf(1.0f, clip_max_norm / (norm + 1e-6f));
   }
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const float ob1 = 1.0f - beta1, ob2 = 1.0f - beta2;
+  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // concatenated float4 index
+  long long end4 = 0;
+  for (int s = 0; s < n_seg; ++s) {
+    const long long delta4 = (__ldg(seg + 3 * s) >> 2) - end4;      // buffer index - concatenated
+    end4 += __ldg(seg + 3 * s + 1) >> 2;
+    if (i >= end4) continue;
+    const int grp = (int)__ldg(seg + 3 * s + 2);
+    const float step_size = groups.step_size[grp], lr_wd = groups.lr_wd[grp];
+    for (; i < end4; i += stride)
+      adamw_vec4(p, g, m, v, p_bf16, i + delta4, step_size, beta1, beta2, ob1, ob2, eps, lr_wd,
+                 grad_scale);
+  }
+}
+
+__global__ void __launch_bounds__(256)
+sumsq_segments_kernel(const float* __restrict__ x, const long long* __restrict__ seg, int n_seg,
+                      float* __restrict__ out) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  float acc = 0.f;
+  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  long long end4 = 0;
+  for (int s = 0; s < n_seg; ++s) {
+    const long long delta4 = (__ldg(seg + 3 * s) >> 2) - end4;
+    end4 += __ldg(seg + 3 * s + 1) >> 2;
+    for (; i < end4; i += stride) {
+      const float4 t = __ldg(reinterpret_cast<const float4*>(x) + i + delta4);
+      acc = fmaf(t.x, t.x, acc); acc = fmaf(t.y, t.y, acc);
+      acc = fmaf(t.z, t.z, acc); acc = fmaf(t.w, t.w, acc);
+    }
+  }
+  block_sum_atomic_add(acc, out);
 }
 
 // Finish of the fused LM-head cross entropy: combine the (max, sum exp) partials of a row.
@@ -158,6 +228,89 @@ extern "C" int hero_adamw_step(float* p, const float* g, float* m, float* v, voi
   adamw_kernel<<<(unsigned)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       p, g, m, v, reinterpret_cast<__nv_bfloat16*>(p_bf16), n, step_size, beta1, beta2, eps, lr_wd,
       grad_scale, clip_sumsq, clip_max_norm);
+  HERO_LAUNCH_CHECK();
+  return HERO_OK;
+}
+
+// Host-side checks of a segment table; sets *total4 to the float4 count over all segments.
+static int check_segments(const int64_t* seg, int32_t n_seg, int64_t n, int32_t n_groups,
+                          long long* total4) {
+  HERO_REQUIRE(n_groups >= 1 && n_groups <= HERO_ADAMW_MAX_GROUPS,
+               "segments: %d groups (1 to %d supported)", n_groups, HERO_ADAMW_MAX_GROUPS);
+  HERO_REQUIRE(n_seg >= 0 && (seg != nullptr || n_seg == 0), "segments: bad table");
+  long long sum = 0, end = 0;
+  for (int32_t s = 0; s < n_seg; ++s) {
+    const int64_t st = seg[3 * s], len = seg[3 * s + 1], grp = seg[3 * s + 2];
+    HERO_REQUIRE(grp >= 0 && grp < n_groups, "segments: segment %d has group %lld, not in [0, %d)",
+                 s, (long long)grp, n_groups);
+    HERO_REQUIRE(st >= 0 && len >= 0 && len <= n - st,
+                 "segments: segment %d = [%lld, %lld + %lld) is not inside [0, %lld)", s,
+                 (long long)st, (long long)st, (long long)len, (long long)n);
+    HERO_REQUIRE(st % 4 == 0 && len % 4 == 0,
+                 "segments: segment %d: start and length must be multiples of 4", s);
+    HERO_REQUIRE(st >= end, "segments: segment %d overlaps or precedes the previous one", s);
+    end = st + len;
+    sum += len;
+  }
+  *total4 = sum / 4;
+  return HERO_OK;
+}
+
+static long long stream_blocks(long long n4, int sms) {
+  long long blocks = (n4 + 255) / 256;
+  if (blocks < 1) blocks = 1;
+  if (blocks > sms * 8LL) blocks = sms * 8LL;
+  return blocks;
+}
+
+extern "C" int hero_adamw_step_groups(float* p, const float* g, float* m, float* v, void* p_bf16,
+                                      int64_t n, const int64_t* segments_host,
+                                      const int64_t* segments_dev, int32_t n_segments,
+                                      const hero_adamw_groups* groups, float beta1, float beta2,
+                                      float eps, float grad_scale, const float* clip_sumsq,
+                                      float clip_max_norm, void* stream) {
+  HERO_REQUIRE(p && g && m && v && groups && n >= 0, "adamw_groups: bad args");
+  HERO_REQUIRE(((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) |
+                 reinterpret_cast<uintptr_t>(m) | reinterpret_cast<uintptr_t>(v)) & 15u) == 0 &&
+                   (reinterpret_cast<uintptr_t>(p_bf16) & 7u) == 0,
+               "adamw_groups: buffers must be 16-byte aligned (bf16 copy 8-byte)");
+  long long total4 = 0;
+  const int st = check_segments(segments_host, n_segments, n, groups->n_groups, &total4);
+  if (st != HERO_OK) return st;
+  HERO_REQUIRE(segments_dev != nullptr || n_segments == 0, "adamw_groups: no device table");
+  if (total4 == 0) return HERO_OK;
+  const int sms = sm_count();
+  if (sms <= 0) return set_error(HERO_ERR_NO_DEVICE, "no CUDA device");
+  AdamwGroupArgs ga;
+  for (int k = 0; k < HERO_ADAMW_MAX_GROUPS; ++k) {
+    ga.step_size[k] = k < groups->n_groups ? groups->step_size[k] : 0.f;
+    ga.lr_wd[k] = k < groups->n_groups ? groups->lr_wd[k] : 0.f;
+  }
+  adamw_groups_kernel<<<(unsigned)stream_blocks(total4, sms), 256, 0,
+                        reinterpret_cast<cudaStream_t>(stream)>>>(
+      p, g, m, v, reinterpret_cast<__nv_bfloat16*>(p_bf16),
+      reinterpret_cast<const long long*>(segments_dev), n_segments, ga, beta1, beta2, eps,
+      grad_scale, clip_sumsq, clip_max_norm);
+  HERO_LAUNCH_CHECK();
+  return HERO_OK;
+}
+
+extern "C" int hero_sumsq_segments_f32(const float* x, int64_t n, const int64_t* segments_host,
+                                       const int64_t* segments_dev, int32_t n_segments,
+                                       int32_t n_groups, float* out, void* stream) {
+  HERO_REQUIRE(x && out && n >= 0, "sumsq_segments: bad args");
+  HERO_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15u) == 0,
+               "sumsq_segments: x must be 16-byte aligned");
+  long long total4 = 0;
+  const int st = check_segments(segments_host, n_segments, n, n_groups, &total4);
+  if (st != HERO_OK) return st;
+  HERO_REQUIRE(segments_dev != nullptr || n_segments == 0, "sumsq_segments: no device table");
+  if (total4 == 0) return HERO_OK;
+  const int sms = sm_count();
+  if (sms <= 0) return set_error(HERO_ERR_NO_DEVICE, "no CUDA device");
+  sumsq_segments_kernel<<<(unsigned)stream_blocks(total4, sms), 256, 0,
+                          reinterpret_cast<cudaStream_t>(stream)>>>(
+      x, reinterpret_cast<const long long*>(segments_dev), n_segments, out);
   HERO_LAUNCH_CHECK();
   return HERO_OK;
 }

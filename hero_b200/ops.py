@@ -464,6 +464,78 @@ def adamw_step(p, g, m, v, p_bf16, *, step_size, beta1, beta2, eps, lr_wd, grad_
                                           grad_scale, _ptr(clip_sumsq), clip_max_norm, _stream()))
 
 
+ADAMW_MAX_GROUPS = _lib.ADAMW_MAX_GROUPS
+
+
+class SegmentTable:
+    """Disjoint ranges of a flat buffer of `n` elements, each in one of `n_groups` parameter
+    groups: the int64 (start, length, group) table of `hero_adamw_step_groups` /
+    `hero_sumsq_segments_f32`, sorted by start, kept on the host for the per-call argument checks
+    and uploaded once to `device`. Raises ValueError for what the kernels refuse: more than
+    ADAMW_MAX_GROUPS groups, a group out of range, a segment outside [0, n), a start or length
+    that is not a multiple of 4, overlapping segments."""
+
+    def __init__(self, segments, n, n_groups, device):
+        if not 1 <= n_groups <= ADAMW_MAX_GROUPS:
+            raise ValueError(f"segment table: {n_groups} groups; the kernels take 1 to "
+                             f"{ADAMW_MAX_GROUPS}")
+        segs = sorted((int(a), int(length), int(grp)) for a, length, grp in segments)
+        end = 0
+        for a, length, grp in segs:
+            if not 0 <= grp < n_groups:
+                raise ValueError(f"segment table: group {grp} not in [0, {n_groups})")
+            if a < 0 or length < 0 or a + length > n:
+                raise ValueError(f"segment table: [{a}, {a + length}) is not inside [0, {n})")
+            if a % 4 or length % 4:
+                raise ValueError(f"segment table: [{a}, {a + length}): start and length must be "
+                                 "multiples of 4")
+            if a < end:
+                raise ValueError(f"segment table: [{a}, {a + length}) overlaps a previous segment")
+            end = a + length
+        self.n, self.n_groups, self.n_segments = int(n), int(n_groups), len(segs)
+        self.covered = sum(length for _, length, _ in segs)   # elements in some segment
+        self.host = torch.tensor(segs, dtype=torch.int64).reshape(-1, 3).contiguous()
+        self.dev = self.host.to(device)
+
+    def _check(self, x):
+        if x.numel() != self.n:
+            raise ValueError(f"segment table describes {self.n} elements, the buffer has "
+                             f"{x.numel()}")
+
+
+def adamw_step_groups(p, g, m, v, p_bf16, table, *, step_sizes, lr_wds, beta1, beta2, eps,
+                      grad_scale=1.0, clip_sumsq=None, clip_max_norm=0.0):
+    """`adamw_step` over every segment of `table` (a SegmentTable) in ONE launch, segment i with
+    step_sizes[group] / lr_wds[group] of its group; bitwise the result of one adamw_step per
+    segment. Elements outside the segments are not touched."""
+    _require_cuda(p, g, m, v, p_bf16)
+    table._check(p)
+    if len(step_sizes) != table.n_groups or len(lr_wds) != table.n_groups:
+        raise ValueError(f"adamw_step_groups: {len(step_sizes)} step sizes / {len(lr_wds)} "
+                         f"lr_wd values for {table.n_groups} groups")
+    grp = _lib.AdamwGroups()
+    grp.n_groups = table.n_groups
+    for k in range(table.n_groups):
+        grp.step_size[k] = step_sizes[k]
+        grp.lr_wd[k] = lr_wds[k]
+    _count()
+    _lib.check(_lib.lib().hero_adamw_step_groups(
+        _ptr(p), _ptr(g), _ptr(m), _ptr(v), _ptr(p_bf16), p.numel(), _ptr(table.host),
+        _ptr(table.dev), table.n_segments, C.byref(grp), beta1, beta2, eps, grad_scale,
+        _ptr(clip_sumsq), clip_max_norm, _stream()))
+
+
+def sumsq_segments(x, table, out):
+    """out += sum of x^2 over the segments of `table` (a SegmentTable)."""
+    _require_cuda(x, out)
+    table._check(x)
+    _count()
+    _lib.check(_lib.lib().hero_sumsq_segments_f32(_ptr(x), x.numel(), _ptr(table.host),
+                                                  _ptr(table.dev), table.n_segments,
+                                                  table.n_groups, _ptr(out), _stream()))
+    return out
+
+
 def reduce_slots(dst, slots, n_slots, slot_stride, scale, max_ctas=16):
     """dst = (dst + sum of n_slots slices of `slots`, slot_stride apart) * scale, fp32, in place."""
     _require_cuda(dst, slots)

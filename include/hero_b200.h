@@ -421,6 +421,33 @@ int hero_ce_finish(const void* ce_partial, int64_t ld_partial, int32_t n_slabs,
 /* out[0] += sum x^2 (global-norm clipping, train_vcmr.py:258-259). */
 int hero_sumsq_f32(const float* x, int64_t n, float* out, void* stream);
 
+/* Parameter groups (optim/misc.py:14-50: top / v_encoder x decay / no-decay, each with its own lr
+ * and weight decay). A segment table is n_segments int64 triples (start, length, group): disjoint
+ * ranges of the flat buffer in ascending order, start and length multiples of 4, inside [0, n),
+ * group in [0, n_groups). `segments_host` is read on the host for the argument checks (no device
+ * read, no synchronisation); `segments_dev` is the same table in device memory, read by the kernel.
+ * Elements outside every segment (frozen parameters, padding of no group) are neither read nor
+ * written. */
+#define HERO_ADAMW_MAX_GROUPS 8
+typedef struct hero_adamw_groups {
+  int32_t n_groups;                         /* 1..HERO_ADAMW_MAX_GROUPS */
+  float step_size[HERO_ADAMW_MAX_GROUPS];   /* lr * sqrt(1 - b2^t) / (1 - b1^t) of each group */
+  float lr_wd[HERO_ADAMW_MAX_GROUPS];       /* lr * weight_decay of each group */
+} hero_adamw_groups;
+/* One launch: every segment updated as by hero_adamw_step over that range with its group's
+ * step_size / lr_wd (bitwise the same result). The group values travel as kernel arguments, so a
+ * step with new learning rates makes no host-to-device copy. */
+int hero_adamw_step_groups(float* p, const float* g, float* m, float* v, void* p_bf16, int64_t n,
+                           const int64_t* segments_host, const int64_t* segments_dev,
+                           int32_t n_segments, const hero_adamw_groups* groups, float beta1,
+                           float beta2, float eps, float grad_scale, const float* clip_sumsq,
+                           float clip_max_norm, void* stream);
+/* out[0] += sum of x^2 over the segments of the table (clipping over the optimizer's parameters
+ * only); the group column is checked against n_groups as above. */
+int hero_sumsq_segments_f32(const float* x, int64_t n, const int64_t* segments_host,
+                            const int64_t* segments_dev, int32_t n_segments, int32_t n_groups,
+                            float* out, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Video-subtitle matching / moment-retrieval head (SURVEY.md §8f rank 1): the ops that follow the
  * encoder in HeroForPretraining / HeroForVcmr.
