@@ -153,6 +153,8 @@ def _declare(lib):
         f32, f32, f32, f32, vp, f32, vp)
     sig("hero_sumsq_segments_f32", vp, i64, vp, vp, i32, i32, vp, vp)
     sig("hero_ce_finish", vp, i64, i32, vp, i32, vp, vp, vp)
+    sig("hero_ce_finish_stats", vp, i64, i32, vp, i32, vp, vp, vp, vp, vp, vp)
+    sig("hero_row_l2_cos", vp, i64, vp, i64, i32, i32, f32, vp, vp, vp, vp, vp)
     sig("hero_reduce_slots_f32", vp, vp, i32, i64, i64, f32, i32, vp)
     sig("hero_l2norm_split_f32", vp, i64, i32, f32, vp, vp, vp, vp)
     sig("hero_vsm_masked_max", vp, i64, vp, i32, i32, i32, vp, vp, vp)

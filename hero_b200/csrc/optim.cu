@@ -156,13 +156,11 @@ sumsq_segments_kernel(const float* __restrict__ x, const long long* __restrict__
   block_sum_atomic_add(acc, out);
 }
 
-// Finish of the fused LM-head cross entropy: combine the (max, sum exp) partials of a row.
-__global__ void __launch_bounds__(128)
-ce_finish_kernel(const float2* __restrict__ part, long long ld, int n_slabs,
-                 const float* __restrict__ lab, int m, float* __restrict__ loss,
-                 float* __restrict__ lse) {
-  const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= m) return;
+// Row r of the fused LM-head cross entropy: combines the (max, sum exp) partials of its slabs into
+// (row max, log-sum-exp). Shared by ce_finish_kernel and ce_finish_stats_kernel, so both compute
+// bitwise the same lse and loss.
+__device__ __forceinline__ float2 ce_row_finish(const float2* __restrict__ part, long long ld,
+                                                int n_slabs, int r) {
   float mx = -INFINITY;
   for (int t = 0; t < n_slabs; ++t) mx = fmaxf(mx, part[(long long)t * ld + r].x);   // coalesced in r
   float s = 0.f;
@@ -170,9 +168,128 @@ ce_finish_kernel(const float2* __restrict__ part, long long ld, int n_slabs,
     const float2 p = part[(long long)t * ld + r];
     s += p.y * __expf(p.x - mx);
   }
-  const float l = mx + __logf(s);
+  return make_float2(mx, mx + __logf(s));
+}
+
+// Finish of the fused LM-head cross entropy: combine the (max, sum exp) partials of a row.
+__global__ void __launch_bounds__(128)
+ce_finish_kernel(const float2* __restrict__ part, long long ld, int n_slabs,
+                 const float* __restrict__ lab, int m, float* __restrict__ loss,
+                 float* __restrict__ lse) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= m) return;
+  const float l = ce_row_finish(part, ld, n_slabs, r).y;
   lse[r] = l;
   loss[r] = l - lab[r];
+}
+
+// acc[0] += sum_{r < m} a[r], acc[1] += sum_{r < m} b[r], in an order fixed by m and blockDim
+// alone: every CTA has written its rows of a / b; the last CTA to finish (ticket on `done`, zeroed
+// before the launch) sums all m rows, thread t taking rows t, t + blockDim, ... in turn, then the
+// fixed butterfly of warp_sum and the warps in index order. No float atomics: two runs on the same
+// inputs give bitwise the same acc.
+template <typename TB>
+__device__ __forceinline__ void last_cta_accumulate(const float* a, const TB* b, int m,
+                                                    float* __restrict__ acc,
+                                                    unsigned* __restrict__ done) {
+  __shared__ bool last;
+  __shared__ float wsum[2][32];
+  __threadfence();                       // this CTA's rows of a / b are visible device-wide
+  __syncthreads();
+  if (threadIdx.x == 0) last = atomicAdd(done, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  float sa = 0.f, sb = 0.f;
+  for (int r = threadIdx.x; r < m; r += blockDim.x) {
+    sa += __ldcg(a + r);                 // L2: the rows were written by other SMs
+    sb += (float)__ldcg(b + r);
+  }
+  sa = warp_sum(sa);
+  sb = warp_sum(sb);
+  const int warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+  if ((threadIdx.x & 31) == 0) {
+    wsum[0][warp] = sa;
+    wsum[1][warp] = sb;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float ta = 0.f, tb = 0.f;
+    for (int w = 0; w < n_warps; ++w) {
+      ta += wsum[0][w];
+      tb += wsum[1][w];
+    }
+    acc[0] += ta;
+    acc[1] += tb;
+  }
+}
+
+// hero_ce_finish plus the top-1 hit of every row and an optional fixed-order accumulation. The
+// label logit is the same fp32 register value that entered its slab's max in the GEMM epilogue, so
+// label_logit >= (max over slabs) holds exactly when the label column is a top-1 column.
+__global__ void __launch_bounds__(128)
+ce_finish_stats_kernel(const float2* __restrict__ part, long long ld, int n_slabs,
+                       const float* __restrict__ lab, int m, float* __restrict__ loss,
+                       float* __restrict__ lse, int* __restrict__ hit, float* __restrict__ acc,
+                       unsigned* __restrict__ done) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r < m) {
+    const float2 f = ce_row_finish(part, ld, n_slabs, r);
+    const float v = lab[r];
+    lse[r] = f.y;
+    loss[r] = f.y - v;
+    hit[r] = v >= f.x ? 1 : 0;
+  }
+  if (acc != nullptr) last_cta_accumulate(loss, hit, m, acc, done);
+}
+
+// Per row of x, y (fp32 [m, d], rows ld apart): l2[r] = sqrt(sum (x - y)^2) and
+// cos[r] = x.y / (max(|x|, eps) * max(|y|, eps)), F.cosine_similarity as torch 2.x computes it
+// (each norm clamped on its own). One warp per row, eight rows per CTA.
+template <bool VEC>
+__global__ void __launch_bounds__(256)
+row_l2_cos_kernel(const float* __restrict__ x, const float* __restrict__ y, int m, int d,
+                  long long ldx, long long ldy, float eps, float* __restrict__ l2,
+                  float* __restrict__ cos_out, float* __restrict__ acc,
+                  unsigned* __restrict__ done) {
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row < m) {
+    const float* xr = x + (long long)row * ldx;
+    const float* yr = y + (long long)row * ldy;
+    float sdd = 0.f, sxx = 0.f, syy = 0.f, sxy = 0.f;
+    if (VEC) {
+      for (int i = lane; i < (d >> 2); i += 32) {
+        const float4 a = __ldg(reinterpret_cast<const float4*>(xr) + i);
+        const float4 b = __ldg(reinterpret_cast<const float4*>(yr) + i);
+        const float xa[4] = {a.x, a.y, a.z, a.w}, yb[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float t = xa[j] - yb[j];
+          sdd = fmaf(t, t, sdd);
+          sxx = fmaf(xa[j], xa[j], sxx);
+          syy = fmaf(yb[j], yb[j], syy);
+          sxy = fmaf(xa[j], yb[j], sxy);
+        }
+      }
+    } else {
+      for (int i = lane; i < d; i += 32) {
+        const float a = __ldg(xr + i), b = __ldg(yr + i), t = a - b;
+        sdd = fmaf(t, t, sdd);
+        sxx = fmaf(a, a, sxx);
+        syy = fmaf(b, b, syy);
+        sxy = fmaf(a, b, sxy);
+      }
+    }
+    sdd = warp_sum(sdd);
+    sxx = warp_sum(sxx);
+    syy = warp_sum(syy);
+    sxy = warp_sum(sxy);
+    if (lane == 0) {
+      l2[row] = sqrtf(sdd);
+      cos_out[row] = sxy / (fmaxf(sqrtf(sxx), eps) * fmaxf(sqrtf(syy), eps));
+    }
+  }
+  if (acc != nullptr) last_cta_accumulate(l2, cos_out, m, acc, done);
 }
 
 // dst[i] = (dst[i] + sum_s slots[s * stride + i]) * scale: the reduction step of the copy-engine
@@ -323,6 +440,47 @@ extern "C" int hero_ce_finish(const void* ce_partial, int64_t ld_partial, int32_
   if (m <= 0) return HERO_OK;
   ce_finish_kernel<<<(m + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const float2*>(ce_partial), ld_partial, n_slabs, label_logit, m, loss, lse);
+  HERO_LAUNCH_CHECK();
+  return HERO_OK;
+}
+
+extern "C" int hero_ce_finish_stats(const void* ce_partial, int64_t ld_partial, int32_t n_slabs,
+                                    const float* label_logit, int32_t m, float* loss, float* lse,
+                                    int32_t* hit, float* acc, uint32_t* counter, void* stream) {
+  HERO_REQUIRE(ce_partial && label_logit && loss && lse && hit && n_slabs > 0 && ld_partial >= m &&
+                   m >= 0 && m <= HERO_ROW_STATS_MAX_ROWS,
+               "ce_finish_stats: bad args (m = %d, at most %d rows)", m, HERO_ROW_STATS_MAX_ROWS);
+  HERO_REQUIRE(acc == nullptr || counter != nullptr, "ce_finish_stats: acc needs a counter");
+  if (m == 0) return HERO_OK;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (acc != nullptr) HERO_CUDA_CHECK(cudaMemsetAsync(counter, 0, sizeof(uint32_t), st));
+  ce_finish_stats_kernel<<<(m + 127) / 128, 128, 0, st>>>(
+      reinterpret_cast<const float2*>(ce_partial), ld_partial, n_slabs, label_logit, m, loss, lse,
+      hit, acc, counter);
+  HERO_LAUNCH_CHECK();
+  return HERO_OK;
+}
+
+extern "C" int hero_row_l2_cos(const float* x, int64_t ldx, const float* y, int64_t ldy, int32_t m,
+                               int32_t d, float eps, float* l2, float* cos, float* acc,
+                               uint32_t* counter, void* stream) {
+  HERO_REQUIRE(m >= 0 && m <= HERO_ROW_STATS_MAX_ROWS && d >= 1 && d <= HERO_ROW_L2_COS_MAX_D,
+               "row_l2_cos: (m, d) = (%d, %d); 0 <= m <= %d and 1 <= d <= %d", m, d,
+               HERO_ROW_STATS_MAX_ROWS, HERO_ROW_L2_COS_MAX_D);
+  HERO_REQUIRE(x && y && l2 && cos && ldx >= d && ldy >= d, "row_l2_cos: bad args");
+  HERO_REQUIRE(acc == nullptr || counter != nullptr, "row_l2_cos: acc needs a counter");
+  if (m == 0) return HERO_OK;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (acc != nullptr) HERO_CUDA_CHECK(cudaMemsetAsync(counter, 0, sizeof(uint32_t), st));
+  const bool vec = d % 4 == 0 && ldx % 4 == 0 && ldy % 4 == 0 &&
+                   ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15u) == 0;
+  const unsigned blocks = (unsigned)((m + 7) / 8);
+  if (vec)
+    row_l2_cos_kernel<true><<<blocks, 256, 0, st>>>(x, y, m, d, ldx, ldy, eps, l2, cos, acc,
+                                                    counter);
+  else
+    row_l2_cos_kernel<false><<<blocks, 256, 0, st>>>(x, y, m, d, ldx, ldy, eps, l2, cos, acc,
+                                                     counter);
   HERO_LAUNCH_CHECK();
   return HERO_OK;
 }

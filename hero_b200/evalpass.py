@@ -17,6 +17,10 @@
   (DESIGN §4 "Temporal NMS and TVR metrics").
 * `validate_videoqa` — eval_videoQA.py:120-173 for one process on HeroForVideoQA.
 * `validate_violin` — eval_violin.py:118-164 for one process on HeroForViolin.
+* `validate_pretrain` (and `validate_mlm` / `_mffr` / `_mfm_nce` / `_fom` / `_vsm`) —
+  pretrain.py:387-608 for one process: the fused LM-head GEMM with `hero_ce_finish_stats` for MLM
+  and MFM-NCE (no logits tensor), `hero_row_l2_cos` for l2 / cosine, sums on the device, one
+  device->host copy per task (DESIGN §4 "Pretraining validation").
 * `ModelSaver` / `TrainingRestorer` — utils/save.py:112-181 with the same file layout (`vocab_padded`
   flag, `model_step_<n>.pt`, `train_state_<n>.pt`, `restore.pt` + backup), so checkpoints are
   interchangeable with the reference's; optimizer state is FusedAdamW's flat moments.
@@ -822,6 +826,258 @@ def validate_violin(model, loader, split, save_logits=False):
                f"valid/{split}_ex_per_s": n_ex / tot_time}
     model.train()
     return val_log, results, logits
+
+
+# ------------------------------------------------------------------ pretraining validation
+# pretrain.py:387-608 for one process. Every metric sum stays in a small fp32 device accumulator;
+# each task makes ONE device->host copy, after its last batch. Example counts come from host-known
+# shapes. Averaging across ranks (all_gather_list) is left to the caller.
+class MlmPlan:
+    # Twin of CrossModalTrm._plan_for (encoder.py) for a batch with frames and text: keep the
+    # two in step.
+    """Packed layout of an MLM batch (data/mlm.py mlm_collate: `attn_masks`, `gather_index`,
+    `v_feat`, `input_ids`), built from its HOST tensors: the layout CrossModalTrm builds from the
+    masks when no plan is given, which reads them back from the device. `attach_mlm_plan` stores
+    it in the batch under plan.PLAN_KEY."""
+
+    def __init__(self, batch):
+        from .plan import FPlan, table_csr
+        max_vl, max_sl = batch["v_feat"].shape[1], batch["input_ids"].shape[1]
+        self.f = FPlan(batch["attn_masks"], batch["gather_index"], max_vl, max_sl)
+        arrays = self.f.arrays("f_")
+        arrays["f_txtpos_off"], arrays["f_txtpos_idx"] = table_csr(self.f.txt_j, max(max_sl, 1))
+        arrays["f_imgpos_off"], arrays["f_imgpos_idx"] = table_csr(self.f.img_k, max(max_vl, 1))
+        self._arrays, self._dev = arrays, {}
+
+    def to(self, device):
+        from .plan import DeviceIndex
+        if device not in self._dev:
+            self._dev[device] = DeviceIndex(self._arrays, device)
+        return self._dev[device]
+
+
+def attach_mlm_plan(batch):
+    """Collate-side hook for MLM batches (plan.attach_plan covers the other pretraining tasks)."""
+    batch[PLAN_KEY] = MlmPlan(batch)
+    return batch
+
+
+def _f_encoder(model):
+    v_enc = model.v_encoder if hasattr(model, "v_encoder") else model
+    return v_enc.f_encoder if hasattr(v_enc, "f_encoder") else v_enc
+
+
+def _device_of(model):
+    return next(model.parameters()).device
+
+
+def _mlm_batch_stats(model, batch, acc):
+    """The masked tokens of `batch` through the encoder and the LM-head transform exactly as
+    CrossModalTrm.forward_mlm runs them, then the fused vocabulary GEMM with
+    `ops.lm_head_ce_stats`: acc += (sum of the token losses, number of top-1 hits), and no
+    (n_masked, V) logits tensor."""
+    # Twin of CrossModalTrm.forward_mlm (encoder.py: plan, packed encoder, masked-token selection,
+    # LM-head transform), with a plan argument and the stats GEMM in place of the loss: a change
+    # to either must be made to both.
+    from .layers import gelu
+    from .params import flat_of
+    fe = _f_encoder(model)
+    input_ids, img_feat = batch["input_ids"], batch.get("v_feat")
+    fplan, dev, pos_keys = fe._plan_for(input_ids, img_feat, batch["attn_masks"],
+                                        batch.get("gather_index"), batch.get(PLAN_KEY))
+    y = fe.encode_packed(fplan, dev, input_ids, batch.get("position_ids"), img_feat,
+                         batch.get("f_pos_ids"), pos_keys=pos_keys, out_f32=True)
+    labels = batch["txt_labels"]
+    n = int(labels.shape[0])
+    if n == 0:
+        return 0
+    tgt = batch["txt_mask_tgt"].to(y.device, non_blocking=True)
+    flat_idx = torch.nonzero_static(tgt.reshape(-1), size=n).reshape(-1)
+    tok = dev.f_pad_to_tok.long()[flat_idx]
+    head = fe.lm_head
+    h = head.LayerNorm(gelu(head.dense(y[tok].to(head.dense.weight.dtype))))
+    emb = fe.embeddings.word_embeddings.weight
+    ops.lm_head_ce_stats(h.to(torch.bfloat16).contiguous(), flat_of(fe, h.device).bf16(emb),
+                         head.bias.detach().float().contiguous(),
+                         labels.to(device=h.device, dtype=torch.int32), emb.shape[0] - fe.vocab_pad,
+                         acc=acc)
+    return n
+
+
+@torch.no_grad()
+def validate_mlm(model, val_loader):
+    """pretrain.py:436-461: {'loss': summed token cross entropy / n_word, 'acc': top-1 hits /
+    n_word, 'tok_per_s'}. Stated deviation: a label tied with another column for the row maximum
+    counts as a hit (the reference's torch.max reports one index of the tie)."""
+    import time
+    t0 = time.time()
+    acc = torch.zeros(2, dtype=torch.float32, device=_device_of(model))
+    n_word = 0
+    for batch in val_loader:
+        n_word += _mlm_batch_stats(model, batch, acc)
+    val_loss, n_correct = acc.cpu().tolist()
+    tot_time = time.time() - t0
+    return {"loss": val_loss / n_word, "acc": n_correct / n_word, "tok_per_s": n_word / tot_time}
+
+
+@torch.no_grad()
+def validate_mffr(model, val_loader):
+    """pretrain.py:464-490: {'loss': sum over masked frames of sqrt(sum (pred - target)^2) /
+    n_feat, 'cosine': summed cosine similarity / n_feat, 'feat_per_s'}; both sums come from
+    `ops.row_l2_cos`. As in the reference, forward_mfm zeroes the masked frames of the batch's
+    c_v_feats in place."""
+    import time
+    t0 = time.time()
+    acc = torch.zeros(2, dtype=torch.float32, device=_device_of(model))
+    n_feat = 0
+    for batch in val_loader:
+        targets = batch["feat_targets"]
+        pred = model(batch, task="mffr", compute_loss=False)
+        if targets.shape[0]:
+            ops.row_l2_cos(pred.float().contiguous(), targets.float().contiguous(), acc=acc)
+        n_feat += int(targets.shape[0])
+    val_loss, cosine = acc.cpu().tolist()
+    tot_time = time.time() - t0
+    return {"loss": val_loss / n_feat, "cosine": cosine / n_feat, "feat_per_s": n_feat / tot_time}
+
+
+def _nce_batch_stats(pred, pos, neg, acc_ce, acc_l2):
+    """MFM-NCE logits pred @ [pos; neg]^T (no temperature, as model.mfm_nce(compute_loss=False))
+    through the fused cross-entropy GEMM with labels arange(n): bf16 operands, B zero-padded to a
+    multiple of 8 rows that ce_n_valid excludes, no bias. l2 / cosine of pred against pos."""
+    n, d = pred.shape
+    n_cols = n + neg.shape[0]
+    b = torch.zeros(((n_cols + 7) // 8 * 8, d), dtype=torch.bfloat16, device=pred.device)
+    b[:n] = pos
+    b[n:n_cols] = neg
+    labels = torch.arange(n, dtype=torch.int32, device=pred.device)
+    ops.lm_head_ce_stats(pred.to(torch.bfloat16).contiguous(), b, None, labels, n_cols, acc=acc_ce)
+    ops.row_l2_cos(pred.float().contiguous(), pos.float().contiguous(), acc=acc_l2)
+
+
+@torch.no_grad()
+def validate_mfm_nce(model, val_loader):
+    """pretrain.py:493-543: {'loss', 'acc', 'l2', 'cosine', 'feat_per_s'}, every sum divided by
+    n_feat. The logits never exist: the fused cross-entropy GEMM keeps online-softmax partials
+    and the hit of every row (an exact tie with the label counts as a hit). Its operands are bf16:
+    the NCE loss differs from the reference's fp32 logits by the bf16 rounding of pred and of the
+    targets (DESIGN §4 "Pretraining validation")."""
+    import time
+    t0 = time.time()
+    dev = _device_of(model)
+    acc_ce = torch.zeros(2, dtype=torch.float32, device=dev)
+    acc_l2 = torch.zeros(2, dtype=torch.float32, device=dev)
+    n_feat = 0
+    for batch in val_loader:
+        pos = batch["feat_targets"]
+        feats, neg_feats = model(batch, task="mfm-nce", compute_loss=False)
+        if pos.shape[0]:
+            _nce_batch_stats(feats, pos, neg_feats, acc_ce, acc_l2)
+        n_feat += int(pos.shape[0])
+    val_loss, n_correct, val_l2, cosine = torch.cat([acc_ce, acc_l2]).cpu().tolist()
+    tot_time = time.time() - t0
+    return {"loss": val_loss / n_feat, "acc": n_correct / n_feat, "l2": val_l2 / n_feat,
+            "cosine": cosine / n_feat, "feat_per_s": n_feat / tot_time}
+
+
+def _host_mask(plan):
+    """The (B, T) clip mask of a ReprPlan, rebuilt on the host from its packed positions."""
+    seq = plan.c.seq
+    mask = np.zeros((seq.rows, seq.length), dtype=np.int64)
+    mask[seq.tok_row, seq.tok_col] = 1
+    return torch.from_numpy(mask)
+
+
+@torch.no_grad()
+def validate_fom(model, val_loader):
+    """pretrain.py:546-589: {'valid/loss': cross entropy summed over the rows whose target is not
+    -1 / their count, 'valid/acc': top-1 hits on those rows / their count, 'valid/ex_per_s'}.
+    Unlike the reference (pretrain.py:577-578) the batch is not mutated: `targets` and `vids` are
+    left in it. With a plan attached, the temporal pass reads its clip mask from the plan instead
+    of the device."""
+    import time
+    t0 = time.time()
+    acc = torch.zeros(3, dtype=torch.float32, device=_device_of(model))
+    n_ex = 0
+    for batch in val_loader:
+        b = {k: v for k, v in batch.items() if k not in ("targets", "vids")}
+        if b.get(PLAN_KEY) is not None:
+            b["c_attn_masks"] = _host_mask(b[PLAN_KEY])
+        scores = model(b, task="fom", compute_loss=False)
+        targets = batch["targets"].to(scores.device, non_blocking=True).reshape(scores.shape[0])
+        valid = targets != -1
+        loss = torch.nn.functional.cross_entropy(scores.float(), targets, ignore_index=-1,
+                                                 reduction="sum")
+        hits = ((scores.argmax(dim=-1) == targets) & valid).sum()
+        acc += torch.stack([loss, hits.float(), valid.sum().float()])
+        n_ex += len(batch["vids"])
+    val_loss, tot_score, n_valid_ex = acc.cpu().tolist()
+    tot_time = time.time() - t0
+    return {"valid/loss": val_loss / n_valid_ex, "valid/acc": tot_score / n_valid_ex,
+            "valid/ex_per_s": n_ex / tot_time}
+
+
+@torch.no_grad()
+def validate_vsm(model, val_loader, opts):
+    """pretrain.py:409-433: model(batch, 'vsm', compute_loss=True) in eval mode ('sum'
+    reductions), the three loss sums accumulated on the device; n_ex = len(q_vidx), the positives
+    counted from loss_neg_ctx's shape. Normalised by opts.lw_st_ed / lw_neg_ctx / lw_neg_q as the
+    reference does."""
+    import time
+    t0 = time.time()
+    acc = torch.zeros(3, dtype=torch.float32, device=_device_of(model))
+    use_neg = opts.lw_neg_ctx != 0 or opts.lw_neg_q != 0
+    n_ex, n_ex_pos = 0, 0
+    for batch in val_loader:
+        n_ex += len(batch["q_vidx"])
+        loss_st_ed, loss_neg_ctx, loss_neg_q = model(batch, "vsm", compute_loss=True)
+        parts = [loss_st_ed.sum()]
+        if use_neg:
+            parts += [loss_neg_ctx.sum(), loss_neg_q.sum()]
+            n_ex_pos += loss_neg_ctx.numel()
+        acc[:len(parts)] += torch.stack(parts).float()
+    val_loss_st_ed, val_loss_neg_ctx, val_loss_neg_q = acc.cpu().tolist()
+    tot_time = time.time() - t0
+    if opts.lw_st_ed:
+        val_loss_st_ed /= n_ex
+        val_loss_st_ed /= opts.lw_st_ed
+    if n_ex_pos > 0 and opts.lw_neg_q > 0 and opts.lw_neg_ctx > 0:
+        val_loss_neg_ctx /= n_ex_pos
+        val_loss_neg_q /= n_ex_pos
+        val_loss_neg_ctx /= opts.lw_neg_ctx
+        val_loss_neg_q /= opts.lw_neg_q
+    val_loss = (opts.lw_st_ed * val_loss_st_ed + opts.lw_neg_ctx * val_loss_neg_ctx +
+                opts.lw_neg_q * val_loss_neg_q)
+    return {"valid/loss_overall": val_loss, "valid/loss_st_ed": val_loss_st_ed,
+            "valid/loss_neg_ctx": val_loss_neg_ctx, "valid/loss_neg_q": val_loss_neg_q,
+            "valid/ex_per_s": n_ex / tot_time}
+
+
+def validate_pretrain(model, val_dataloaders, opts):
+    """pretrain.py:387-406 (validate) for one process: model.eval(), each task's validation
+    chosen by the prefix of its name ('mlm', 'mffr', 'mfm-nce', 'fom', 'vsm'), model.train() on
+    exit. Returns the dict the reference logs, {f'{task}_{k}': v} over all tasks. `opts` needs
+    lw_st_ed, lw_neg_ctx and lw_neg_q. Raises ValueError for an unknown task."""
+    model.eval()
+    out = {}
+    try:
+        for task, loader in val_dataloaders.items():
+            if task.startswith("mlm"):
+                val_log = validate_mlm(model, loader)
+            elif task.startswith("mffr"):
+                val_log = validate_mffr(model, loader)
+            elif task.startswith("mfm-nce"):
+                val_log = validate_mfm_nce(model, loader)
+            elif task.startswith("fom"):
+                val_log = validate_fom(model, loader)
+            elif task.startswith("vsm"):
+                val_log = validate_vsm(model, loader, opts)
+            else:
+                raise ValueError(f"Undefined task {task}")
+            out.update({f"{task}_{k}": v for k, v in val_log.items()})
+    finally:
+        model.train()
+    return out
 
 
 def decode_tvc(model, loader, *, max_step, bos, eos, tokenizer):

@@ -671,10 +671,11 @@ def temporal_nms(score, mom, n_in, thd, interval, by_clip, n_out, out_score, out
 
 # ---------------------------------------------------------------------------------------------
 # Fused LM-head cross entropy (MLM): vocabulary logits are never materialised in fp32.
-def lm_head_ce_fwd(h, emb, bias, labels, n_valid):
-    """h: bf16 [n, H] (LM-head transform of the masked tokens), emb: bf16 [V, H] (tied word
-    embedding), bias: fp32 [V], labels: int32 [n]. Returns (loss fp32 [n], lse fp32 [n]) of
-    F.cross_entropy(h @ emb.T + bias, labels, reduction='none') over the first n_valid columns."""
+def lm_head_ce_partials(h, emb, bias, labels, n_valid):
+    """The act-4 GEMM of the fused cross entropy alone. h: bf16 [n, K], emb: bf16 [V, K] (V a
+    multiple of 8), bias: fp32 [V] or None, labels: int32 [n]. Returns (partial fp32
+    [ceil(V / 64), ld, 2]: per 64-column slab and row the (max, sum exp) over the columns below
+    n_valid, label_logit fp32 [n]), which `ce_finish` / `ce_finish_stats` combine."""
     _require_cuda(h, emb, bias, labels)
     assert h.dtype == BF16 and emb.dtype == BF16 and labels.dtype == torch.int32
     n, V = h.shape[0], emb.shape[0]
@@ -691,13 +692,95 @@ def lm_head_ce_fwd(h, emb, bias, labels, n_valid):
     g.drop_scale = 1.0
     g.ce_label, g.ce_partial, g.ce_label_logit = _ptr(labels), _ptr(partial), _ptr(lab)
     g.ce_ld_partial, g.ce_n_valid = ld, n_valid
-    _count(2)
+    _count()
     _lib.check(_lib.lib().hero_gemm_bf16(C.byref(g), _stream()))
-    loss = torch.empty(n, dtype=torch.float32, device=h.device)
-    lse = torch.empty(n, dtype=torch.float32, device=h.device)
-    _lib.check(_lib.lib().hero_ce_finish(_ptr(partial), ld, n_slabs, _ptr(lab), n, _ptr(loss),
-                                         _ptr(lse), _stream()))
+    return partial, lab
+
+
+def ce_finish(partial, label_logit):
+    """(loss fp32 [n], lse fp32 [n]) from the partials of `lm_head_ce_partials` (`hero_ce_finish`)."""
+    n = label_logit.numel()
+    loss = torch.empty(n, dtype=torch.float32, device=partial.device)
+    lse = torch.empty(n, dtype=torch.float32, device=partial.device)
+    _count()
+    _lib.check(_lib.lib().hero_ce_finish(_ptr(partial), partial.shape[1], partial.shape[0],
+                                         _ptr(label_logit), n, _ptr(loss), _ptr(lse), _stream()))
     return loss, lse
+
+
+ROW_STATS_MAX_ROWS = 1 << 24     # HERO_ROW_STATS_MAX_ROWS
+ROW_L2_COS_MAX_D = 4352          # HERO_ROW_L2_COS_MAX_D (vfeat_dim)
+
+
+def _row_stats_bounds(name, m, d=None):
+    if not 0 <= m <= ROW_STATS_MAX_ROWS or (d is not None and not 1 <= d <= ROW_L2_COS_MAX_D):
+        raise ValueError(f"{name}: (m, d) = ({m}, {d}); the kernel takes 0 <= m <= "
+                         f"{ROW_STATS_MAX_ROWS} rows" +
+                         ("" if d is None else f" of 1 <= d <= {ROW_L2_COS_MAX_D} columns"))
+
+
+def _acc_args(acc, device):
+    """(acc, 4-byte counter scratch) for the fixed-order accumulation of the row-stats kernels."""
+    if acc is None:
+        return None, None
+    assert acc.dtype == torch.float32 and acc.is_contiguous() and acc.numel() == 2
+    return acc, torch.empty(1, dtype=torch.int32, device=device)
+
+
+def ce_finish_stats(partial, label_logit, acc=None):
+    """`ce_finish` plus hit int32 [n] = 1 where the label column is a top-1 column of its row (an
+    exact tie counts as a hit); `acc` (fp32 [2], optional) += (sum loss, sum hit) in a fixed order
+    (`hero_ce_finish_stats`). Returns (loss, lse, hit)."""
+    n = label_logit.numel()
+    _row_stats_bounds("ce_finish_stats", n)
+    _require_cuda(partial, label_logit, acc)
+    dev = partial.device
+    loss = torch.empty(n, dtype=torch.float32, device=dev)
+    lse = torch.empty(n, dtype=torch.float32, device=dev)
+    hit = torch.empty(n, dtype=torch.int32, device=dev)
+    acc, counter = _acc_args(acc, dev)
+    _count()
+    _lib.check(_lib.lib().hero_ce_finish_stats(
+        _ptr(partial), partial.shape[1], partial.shape[0], _ptr(label_logit), n, _ptr(loss),
+        _ptr(lse), _ptr(hit), _ptr(acc), _ptr(counter), _stream()))
+    return loss, lse, hit
+
+
+def lm_head_ce_fwd(h, emb, bias, labels, n_valid):
+    """h: bf16 [n, H] (LM-head transform of the masked tokens), emb: bf16 [V, H] (tied word
+    embedding), bias: fp32 [V], labels: int32 [n]. Returns (loss fp32 [n], lse fp32 [n]) of
+    F.cross_entropy(h @ emb.T + bias, labels, reduction='none') over the first n_valid columns."""
+    return ce_finish(*lm_head_ce_partials(h, emb, bias, labels, n_valid))
+
+
+def lm_head_ce_stats(h, emb, bias, labels, n_valid, acc=None):
+    """`lm_head_ce_fwd` with the top-1 hit of every row and the optional fixed-order accumulation
+    of `ce_finish_stats`: (loss, lse, hit), and no (n, V) logits tensor. bias may be None."""
+    return ce_finish_stats(*lm_head_ce_partials(h, emb, bias, labels, n_valid), acc=acc)
+
+
+def row_l2_cos(x, y, acc=None, eps=1e-8):
+    """Per row of x, y (fp32 [m, d], unit column stride, d <= ROW_L2_COS_MAX_D): (l2 = sqrt(sum
+    (x - y)^2), cos = F.cosine_similarity(x, y, dim=-1, eps) as torch 2.x defines it), both fp32
+    [m]; `acc` (fp32 [2], optional) += (sum l2, sum cos) in a fixed order (`hero_row_l2_cos`).
+    The bounds are checked here, before the launch."""
+    if x.dim() != 2 or tuple(y.shape) != tuple(x.shape):
+        raise ValueError(f"row_l2_cos: x {tuple(x.shape)} and y {tuple(y.shape)}: expected two "
+                         "[m, d] tensors of one shape")
+    m, d = x.shape
+    _row_stats_bounds("row_l2_cos", m, d)
+    _require_cuda(x, y, acc)
+    for t in (x, y):
+        assert t.dtype == torch.float32 and t.stride(1) == 1
+    dev = x.device
+    l2 = torch.empty(m, dtype=torch.float32, device=dev)
+    cos = torch.empty(m, dtype=torch.float32, device=dev)
+    acc, counter = _acc_args(acc, dev)
+    _count()
+    _lib.check(_lib.lib().hero_row_l2_cos(_ptr(x), x.stride(0), _ptr(y), y.stride(0), m, d, eps,
+                                          _ptr(l2), _ptr(cos), _ptr(acc), _ptr(counter),
+                                          _stream()))
+    return l2, cos
 
 
 def lm_head_ce_dlogits(h, emb, bias, labels, lse, grad, n_valid, out):

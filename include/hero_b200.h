@@ -418,6 +418,29 @@ int hero_reduce_slots_f32(float* dst, const float* slots, int32_t n_slots, int64
  * loss[r] = lse[r] - label_logit[r] (F.cross_entropy, reduction='none'), r < m. */
 int hero_ce_finish(const void* ce_partial, int64_t ld_partial, int32_t n_slabs,
                    const float* label_logit, int32_t m, float* loss, float* lse, void* stream);
+/* Per-row statistics of a validation pass, at most HERO_ROW_STATS_MAX_ROWS rows per call (so a
+ * count summed in fp32 stays exact). `acc` (fp32 [2], optional) is ADDED to in a fixed order: the
+ * last CTA to finish sums the per-row outputs of the call (no float atomics), so two runs on the
+ * same inputs give bitwise the same acc. With acc, `counter` is 4 bytes of device scratch, cleared
+ * on the stream (cudaMemsetAsync) before the launch; the same counter must not serve two calls that
+ * can run at once. */
+#define HERO_ROW_STATS_MAX_ROWS (1 << 24)
+#define HERO_ROW_L2_COS_MAX_D 4352
+/* hero_ce_finish on the same partials (loss and lse bitwise equal to it) plus
+ * hit[r] = (label_logit[r] >= max over the row's slabs): the label logit is the fp32 value that
+ * entered its slab's max in the epilogue, so this is exactly "the label is a top-1 column". On an
+ * exact tie the label counts as a hit (torch.max would report the lowest tied index instead).
+ * acc[0] += sum loss, acc[1] += sum hit. */
+int hero_ce_finish_stats(const void* ce_partial, int64_t ld_partial, int32_t n_slabs,
+                         const float* label_logit, int32_t m, float* loss, float* lse,
+                         int32_t* hit, float* acc, uint32_t* counter, void* stream);
+/* Per row r < m of x, y (fp32, rows ldx / ldy floats apart, 1 <= d <= HERO_ROW_L2_COS_MAX_D):
+ * l2[r] = sqrt(sum_i (x - y)^2) (the MFFR loss / MFM-NCE l2 of pretrain.py:472-474,521-522) and
+ * cos[r] = x.y / (max(|x|, eps) * max(|y|, eps)), F.cosine_similarity(x, y, dim=-1, eps) as torch
+ * 2.x defines it (torch 1.3 clamped |x|^2 |y|^2 at eps^2 instead; the two differ only for rows
+ * whose norm is below eps). One warp per row. acc[0] += sum l2, acc[1] += sum cos. */
+int hero_row_l2_cos(const float* x, int64_t ldx, const float* y, int64_t ldy, int32_t m, int32_t d,
+                    float eps, float* l2, float* cos, float* acc, uint32_t* counter, void* stream);
 /* out[0] += sum x^2 (global-norm clipping, train_vcmr.py:258-259). */
 int hero_sumsq_f32(const float* x, int64_t n, float* out, void* stream);
 
