@@ -20,7 +20,7 @@ from .embed import FrameEmbeddings, ImageEmbeddings, QueryFeatEmbeddings, SubEmb
 from .layers import (BertAttention, BertEncoder, BertLayerNorm, BertLMPredictionHead, BertPooler,
                      LinearLayer, gelu, mask_logits)
 from .params import flat_of
-from .plan import PLAN_KEY, TxtPlan
+from .plan import PLAN_KEY, TxtPlan, plan_inputs
 
 BF16 = torch.bfloat16
 
@@ -205,48 +205,17 @@ class CrossModalTrm(RobertaPreTrainedModel):
                                token_type_ids=txt_type_ids)
 
     # ---- packed hot path -------------------------------------------------------------------
-    def _embed_cfg(self, fplan, dev, drop, input_ids, position_ids, img_feat, img_pos_ids,
-                   img_masks, pos_keys=("f_txtpos_off", "f_txtpos_idx", "f_imgpos_off",
-                                        "f_imgpos_idx"), shared_feats=None):
-        """`shared_feats`: clip-level frame features (B, T, D) to read the frame slots from when
-        the batch carries no `f_v_feats` (plan.ReprPlan maps every packed frame token to its
-        clip frame)."""
-        device = dev.flat.device
-        cfg = {"drop": drop, "n_tok": fplan.seq.n_tok, "n_txt": fplan.n_txt,
-               "n_img": fplan.n_img, "pad_idx": self.embeddings.padding_idx, "img_mask": None}
-        if fplan.n_txt:
-            # token / position ids per packed text token: gathered by the plan on the host when
-            # it saw the id tensors (collate side), else here with a few index kernels
-            pre_ids = getattr(dev, "f_txt_ids", None) if getattr(fplan, "txt_ids", None) \
-                is not None else None
-            pre_pos = getattr(dev, "f_txt_pos", None) if getattr(fplan, "txt_pos", None) \
-                is not None else None
-            src = None
-            if pre_ids is not None:
-                cfg["txt_ids"] = pre_ids
-            else:
-                src = dev.f_txt_src.long()
-                cfg["txt_ids"] = input_ids.reshape(-1)[src].int()
-            if position_ids is None:
-                position_ids = self.embeddings.create_position_ids_from_input_ids(input_ids)
-                pre_pos = None
-            if position_ids.shape[0] == 1 and input_ids.shape[0] != 1:
-                slot_pos = position_ids.reshape(-1)
-                cfg["txt_pos"] = pre_pos if pre_pos is not None else \
-                    slot_pos[dev.f_txt_j.long()].int()
-                cfg["txt_slot_pos"] = slot_pos
-            else:
-                if pre_pos is not None:
-                    cfg["txt_pos"] = pre_pos
-                else:
-                    src = dev.f_txt_src.long() if src is None else src
-                    cfg["txt_pos"] = position_ids.expand_as(input_ids).reshape(-1)[src].int()
-                cfg["txt_slot_pos"] = None       # per-row position ids: atomic table gradient
-            cfg["txt_tok"] = dev.f_txt_tok
-            cfg["txtpos_off"] = getattr(dev, pos_keys[0])
-            cfg["txtpos_idx"] = getattr(dev, pos_keys[1])
+    def _embed_cfg(self, fplan, dev, drop, img_feat, img_masks, shared_feats=None):
+        """Arguments of functional.cross_modal_embed: the plan's index arrays (FPlan.embed_ids)
+        and the frame features. `shared_feats`: clip-level frame features (B, T, D) to read the
+        frame slots from when the batch carries no `f_v_feats` (plan.ReprPlan maps every packed
+        frame token to its clip frame)."""
+        cfg = {"drop": drop, "n_tok": fplan.n_tok, "n_txt": fplan.n_txt, "n_img": fplan.n_img,
+               "pad_idx": self.embeddings.padding_idx, "img_mask": None}
+        for k in ("txt_tok", "txt_ids", "txt_pos", "txtpos_off", "txtpos_idx", "img_tok",
+                  "img_src", "img_pos", "imgpos_off", "imgpos_idx"):
+            cfg[k] = getattr(dev, k)
         if fplan.n_img:
-            img_src = dev.f_img_src
             if img_feat is None:
                 if shared_feats is None:
                     raise ValueError("batch has neither f_v_feats nor c_v_feats for the frame slots")
@@ -256,27 +225,14 @@ class CrossModalTrm(RobertaPreTrainedModel):
                 if not getattr(fplan, "shared_feats_ok", True):
                     raise ValueError("a frame slot marked valid in f_attn_masks is not listed in "
                                      "sub_idx2frame_idx: this batch cannot omit f_v_feats")
-                img_feat, img_src = shared_feats, dev.f_img_src_c
+                img_feat, cfg["img_src"] = shared_feats, dev.img_src_c
             D = img_feat.shape[-1]
             feats = img_feat.reshape(-1, D)
             if feats.dtype != torch.float32:
                 feats = feats.float()
             cfg["img_feats"] = feats.contiguous()
-            cfg["img_src"] = img_src
-            cfg["img_tok"] = dev.f_img_tok
-            if img_pos_ids is None:
-                cfg["img_k"] = dev.f_img_k
-                cfg["img_slot_pos"] = torch.arange(fplan.max_vl, device=device)
-            else:
-                slot_pos = img_pos_ids.reshape(-1)[:fplan.max_vl]
-                pre = getattr(dev, "f_img_kpos", None) if getattr(fplan, "img_kpos", None) \
-                    is not None else None
-                cfg["img_k"] = pre if pre is not None else slot_pos[dev.f_img_k.long()].int()
-                cfg["img_slot_pos"] = slot_pos
             if img_masks is not None:
-                cfg["img_mask"] = img_masks.reshape(-1)[dev.f_img_src.long()].int()
-            cfg["imgpos_off"] = getattr(dev, pos_keys[2])
-            cfg["imgpos_idx"] = getattr(dev, pos_keys[3])
+                cfg["img_mask"] = img_masks.reshape(-1)[dev.img_src.long()].int()
         return cfg
 
     def _embed_params(self, with_img):
@@ -290,68 +246,20 @@ class CrossModalTrm(RobertaPreTrainedModel):
                        i.mask_embedding.weight, i.LayerNorm.weight, i.LayerNorm.bias]
         return params
 
-    def encode_packed(self, fplan, dev, input_ids, position_ids, img_feat=None, img_pos_ids=None,
-                      img_masks=None, drop=None, pos_keys=None, shared_feats=None, out_f32=False):
-        """Embeddings + encoder on packed tokens -> [n_tokens, H], bf16 (feeds further kernels) or
-        fp32 (`out_f32`: the caller unpacks it as the final result)."""
-        device = dev.flat.device
-        flat = flat_of(self, device)
+    def encode_packed(self, fplan, dev, att, img_feat=None, img_masks=None, drop=None,
+                      shared_feats=None, out_f32=False):
+        """Embeddings + encoder on the packed tokens of a plan (its FPlan, or a JointPlan) with
+        device index `dev` and attention plan `att` -> [n_tokens, H], bf16 (feeds further
+        kernels) or fp32 (`out_f32`: the caller unpacks it as the final result)."""
+        flat = flat_of(self, dev.flat.device)
         if drop is None:
             drop = self.encoder.dropout_state()
-        kw = {} if pos_keys is None else {"pos_keys": pos_keys}
-        if shared_feats is not None:
-            kw["shared_feats"] = shared_feats
-        cfg = self._embed_cfg(fplan, dev, drop, input_ids, position_ids, img_feat, img_pos_ids,
-                              img_masks, **kw)
+        cfg = self._embed_cfg(fplan, dev, drop, img_feat, img_masks, shared_feats)
         with_img = fplan.n_img > 0
         if with_img:
             cfg["img_lin_w_bf16"] = flat.bf16(self.img_embeddings.img_linear.weight)
         emb, emb32 = Fn.cross_modal_embed(cfg, self._embed_params(with_img))
-        return self.encoder.forward_packed(emb, fplan.seq.attn(dev, "f_"), drop, x_f32=emb32,
-                                           out_f32=out_f32)
-
-    def encode_packed_joint(self, jplan, rdev, tdev, jdev, batch, txt_batch, drop=None):
-        """One pass of embeddings + encoder over [video rows | query rows] (see plan.JointPlan).
-        Returns the packed bf16 [n_video_tok + n_query_tok, H] output."""
-        device = jdev.flat.device
-        flat = flat_of(self, device)
-        if drop is None:
-            drop = self.encoder.dropout_state()
-        fv, fq = jplan.r.f, jplan.t.f
-        v_ids, q_ids = batch["f_sub_input_ids"], txt_batch["input_ids"]
-        v_pos, q_pos = batch["f_sub_pos_ids"], txt_batch["pos_ids"]
-        cfg_v = self._embed_cfg(fv, rdev, drop, v_ids, v_pos, batch["f_v_feats"],
-                                batch["f_v_pos_ids"], batch["f_v_masks"],
-                                shared_feats=batch["c_v_feats"] if batch["f_v_feats"] is None
-                                else None)
-        cfg_q = self._embed_cfg(fq, tdev, drop, q_ids, q_pos, None, None, None,
-                                pos_keys=("pos_off", "pos_idx", None, None))
-        cfg = dict(cfg_v)
-        cfg["n_tok"], cfg["n_txt"] = jplan.n_tok, jplan.n_txt
-        if "j_txt_ids" in jplan.arr and "j_txt_pos" in jplan.arr:
-            cfg["txt_ids"], cfg["txt_pos"] = jdev.j_txt_ids, jdev.j_txt_pos    # host-gathered
-        else:
-            cfg["txt_ids"] = torch.cat([cfg_v["txt_ids"], cfg_q["txt_ids"]]) if fv.n_txt else \
-                cfg_q["txt_ids"]
-            cfg["txt_pos"] = torch.cat([cfg_v["txt_pos"], cfg_q["txt_pos"]]) if fv.n_txt else \
-                cfg_q["txt_pos"]
-        cfg["txt_tok"] = jdev.j_txt_tok
-        cfg["txtpos_off"], cfg["txtpos_idx"] = jdev.j_txtpos_off, jdev.j_txtpos_idx
-        sv, sq = cfg_v.get("txt_slot_pos"), cfg_q.get("txt_slot_pos")
-        if sv is not None and sq is not None:
-            n = min(sv.numel(), sq.numel())
-            same = jplan.same_slot_pos        # host-side decision of the plan (no device sync)
-            if same is None:                  # plan built from device tensors: compare here
-                same = bool((sv[:n] == sq[:n]).all()) if n else True
-            cfg["txt_slot_pos"] = (sv if sv.numel() >= sq.numel() else sq) if same else None
-        else:
-            cfg["txt_slot_pos"] = None
-        with_img = fv.n_img > 0
-        if with_img:
-            cfg["img_lin_w_bf16"] = flat.bf16(self.img_embeddings.img_linear.weight)
-        cfg["flat"] = flat
-        emb, emb32 = Fn.cross_modal_embed(cfg, self._embed_params(with_img))
-        return self.encoder.forward_packed(emb, jplan.attn(jdev), drop, x_f32=emb32)
+        return self.encoder.forward_packed(emb, att, drop, x_f32=emb32, out_f32=out_f32)
 
     def _unpack(self, y, dev, shape):
         out = Fn.gather_rows(y, dev.f_pad_to_tok, dev.f_tok_flat)
@@ -376,65 +284,66 @@ class CrossModalTrm(RobertaPreTrainedModel):
             return self.forward_mlm(batch["input_ids"], batch["position_ids"], batch["v_feat"],
                                     batch["f_pos_ids"], batch["attn_masks"],
                                     batch["gather_index"], batch["txt_mask_tgt"],
-                                    batch["txt_labels"], compute_loss)
+                                    batch["txt_labels"], compute_loss, _plan=batch[PLAN_KEY])
         else:
             raise ValueError(f"Unrecognized task {task}")
 
-    def _plan_for(self, input_ids, img_feat, attention_mask, gather_index, _plan=None):
-        from .plan import FPlan, DeviceIndex, table_csr
+    def _plan_for(self, input_ids, position_ids, img_feat, img_pos_ids, attention_mask,
+                  gather_index, _plan=None):
+        """(FPlan, device index) of the attached plan, else of a TxtPlan built here (one
+        device->host read of the masks and ids)."""
         if input_ids is None and img_feat is None:
             raise ValueError("Both img_feat and input_dis are None")
-        if isinstance(_plan, TxtPlan):
-            return _plan.f, _plan.to(attention_mask.device), ("pos_off", "pos_idx", None, None)
-        if _plan is not None and hasattr(_plan, "f"):
-            return _plan.f, _plan.to(attention_mask.device), None
-        if img_feat is None:
-            plan = TxtPlan(attention_mask)
-            return plan.f, plan.to(attention_mask.device), ("pos_off", "pos_idx", None, None)
-        if input_ids is not None:
-            assert gather_index is not None
-        max_vl = img_feat.shape[1]
-        max_sl = input_ids.shape[1] if input_ids is not None else 0
-        fplan = FPlan(attention_mask, gather_index, max_vl, max_sl)
-        arrays = fplan.arrays("f_")
-        arrays["f_txtpos_off"], arrays["f_txtpos_idx"] = table_csr(fplan.txt_j, max(max_sl, 1))
-        arrays["f_imgpos_off"], arrays["f_imgpos_idx"] = table_csr(fplan.img_k, max(max_vl, 1))
-        return fplan, DeviceIndex(arrays, attention_mask.device), None
+        if _plan is None:
+            if input_ids is not None and img_feat is not None:
+                assert gather_index is not None
+            _plan = TxtPlan(**plan_inputs({
+                "attn_masks": attention_mask, "input_ids": input_ids, "position_ids": position_ids,
+                "gather_index": None if img_feat is None else gather_index,
+                "f_pos_ids": None if img_feat is None else img_pos_ids, "v_feat": img_feat}, "mlm"))
+        return _plan.f, _plan.to(attention_mask.device)
 
     def forward_repr(self, input_ids, position_ids, img_feat, img_pos_ids, attention_mask,
                      gather_index=None, txt_type_ids=None, img_type_ids=None, img_masks=None,
                      _plan=None):
         if txt_type_ids is not None or img_type_ids is not None:
             raise ValueError("explicit token type ids are not supported (HERO always uses 1)")
-        fplan, dev, pos_keys = self._plan_for(input_ids, img_feat, attention_mask, gather_index,
-                                              _plan)
-        y = self.encode_packed(fplan, dev, input_ids, position_ids, img_feat, img_pos_ids,
-                               img_masks, pos_keys=pos_keys, out_f32=True)
+        fplan, dev = self._plan_for(input_ids, position_ids, img_feat, img_pos_ids,
+                                    attention_mask, gather_index, _plan)
+        y = self.encode_packed(fplan, dev, fplan.seq.attn(dev, "f_"), img_feat, img_masks,
+                               out_f32=True)
         sequence_output = self._unpack(y, dev, attention_mask.shape)
         pooled_output = self.pooler(sequence_output)
         return (sequence_output, pooled_output)
 
     # ---- MLM (model/encoder.py:355-389); head stays torch ('next' row, SURVEY.md §8f) ------
-    def forward_mlm(self, input_ids, position_ids, img_feat, img_pos_ids, attention_mask,
-                    gather_index, txt_mask_tgt, txt_labels=None, compute_loss=True):
-        """model/encoder.py:355-374. The masked tokens are picked straight out of the PACKED encoder
-        output (no padded tensor, no boolean-mask compaction: their count is `txt_labels.shape[0]`,
-        host-known), pass the LM-head transform (dense + gelu + LayerNorm, model/layers.py:336-346)
-        and — when the loss is wanted — the fused vocabulary GEMM + cross entropy
-        (functional.lm_head_cross_entropy): no (n_masked, 50272) logits tensor exists."""
-        fplan, dev, pos_keys = self._plan_for(input_ids, img_feat, attention_mask, gather_index)
-        y = self.encode_packed(fplan, dev, input_ids, position_ids, img_feat, img_pos_ids,
-                               pos_keys=pos_keys, out_f32=True)
-        if txt_labels is not None:
-            n_masked = int(txt_labels.shape[0])
-            flat_idx = torch.nonzero_static(txt_mask_tgt.reshape(-1), size=n_masked).reshape(-1)
+    def mlm_head_input(self, input_ids, position_ids, img_feat, img_pos_ids, attention_mask,
+                       gather_index, txt_mask_tgt, n_masked=None, _plan=None):
+        """LM-head input h of the masked tokens (model/encoder.py:355-370): they are picked
+        straight out of the PACKED encoder output (no padded tensor; with `n_masked`, the
+        host-known number of masked tokens, no boolean-mask compaction either) and pass the
+        LM-head transform (dense + gelu + LayerNorm, model/layers.py:336-346)."""
+        fplan, dev = self._plan_for(input_ids, position_ids, img_feat, img_pos_ids,
+                                    attention_mask, gather_index, _plan)
+        y = self.encode_packed(fplan, dev, fplan.seq.attn(dev, "f_"), img_feat, out_f32=True)
+        tgt = txt_mask_tgt.to(y.device, non_blocking=True).reshape(-1)
+        if n_masked is not None:
+            flat_idx = torch.nonzero_static(tgt, size=n_masked).reshape(-1)
         else:
-            flat_idx = torch.nonzero(txt_mask_tgt.reshape(-1)).reshape(-1)
+            flat_idx = torch.nonzero(tgt).reshape(-1)
         tok = dev.f_pad_to_tok.long()[flat_idx]               # packed row of every masked token
-        masked_output = y[tok]
         head = self.lm_head
-        wdt = head.dense.weight.dtype
-        h = head.LayerNorm(gelu(head.dense(masked_output.to(wdt))))
+        return head.LayerNorm(gelu(head.dense(y[tok].to(head.dense.weight.dtype))))
+
+    def forward_mlm(self, input_ids, position_ids, img_feat, img_pos_ids, attention_mask,
+                    gather_index, txt_mask_tgt, txt_labels=None, compute_loss=True, _plan=None):
+        """model/encoder.py:355-374: `mlm_head_input`, then — when the loss is wanted — the fused
+        vocabulary GEMM + cross entropy (functional.lm_head_cross_entropy): no (n_masked, 50272)
+        logits tensor exists."""
+        h = self.mlm_head_input(input_ids, position_ids, img_feat, img_pos_ids, attention_mask,
+                                gather_index, txt_mask_tgt,
+                                None if txt_labels is None else int(txt_labels.shape[0]), _plan)
+        head = self.lm_head
         if compute_loss:
             flat = flat_of(self, h.device)
             emb = self.embeddings.word_embeddings.weight

@@ -832,34 +832,9 @@ def validate_violin(model, loader, split, save_logits=False):
 # pretrain.py:387-608 for one process. Every metric sum stays in a small fp32 device accumulator;
 # each task makes ONE device->host copy, after its last batch. Example counts come from host-known
 # shapes. Averaging across ranks (all_gather_list) is left to the caller.
-class MlmPlan:
-    # Twin of CrossModalTrm._plan_for (encoder.py) for a batch with frames and text: keep the
-    # two in step.
-    """Packed layout of an MLM batch (data/mlm.py mlm_collate: `attn_masks`, `gather_index`,
-    `v_feat`, `input_ids`), built from its HOST tensors: the layout CrossModalTrm builds from the
-    masks when no plan is given, which reads them back from the device. `attach_mlm_plan` stores
-    it in the batch under plan.PLAN_KEY."""
-
-    def __init__(self, batch):
-        from .plan import FPlan, table_csr
-        max_vl, max_sl = batch["v_feat"].shape[1], batch["input_ids"].shape[1]
-        self.f = FPlan(batch["attn_masks"], batch["gather_index"], max_vl, max_sl)
-        arrays = self.f.arrays("f_")
-        arrays["f_txtpos_off"], arrays["f_txtpos_idx"] = table_csr(self.f.txt_j, max(max_sl, 1))
-        arrays["f_imgpos_off"], arrays["f_imgpos_idx"] = table_csr(self.f.img_k, max(max_vl, 1))
-        self._arrays, self._dev = arrays, {}
-
-    def to(self, device):
-        from .plan import DeviceIndex
-        if device not in self._dev:
-            self._dev[device] = DeviceIndex(self._arrays, device)
-        return self._dev[device]
-
-
 def attach_mlm_plan(batch):
-    """Collate-side hook for MLM batches (plan.attach_plan covers the other pretraining tasks)."""
-    batch[PLAN_KEY] = MlmPlan(batch)
-    return batch
+    """Collate-side hook for MLM batches: plan.attach_plan(batch, "mlm")."""
+    return attach_plan(batch, "mlm")
 
 
 def _f_encoder(model):
@@ -872,33 +847,21 @@ def _device_of(model):
 
 
 def _mlm_batch_stats(model, batch, acc):
-    """The masked tokens of `batch` through the encoder and the LM-head transform exactly as
-    CrossModalTrm.forward_mlm runs them, then the fused vocabulary GEMM with
-    `ops.lm_head_ce_stats`: acc += (sum of the token losses, number of top-1 hits), and no
-    (n_masked, V) logits tensor."""
-    # Twin of CrossModalTrm.forward_mlm (encoder.py: plan, packed encoder, masked-token selection,
-    # LM-head transform), with a plan argument and the stats GEMM in place of the loss: a change
-    # to either must be made to both.
-    from .layers import gelu
+    """The masked tokens of `batch` through CrossModalTrm.mlm_head_input, then the fused
+    vocabulary GEMM with `ops.lm_head_ce_stats`: acc += (sum of the token losses, number of top-1
+    hits), and no (n_masked, V) logits tensor."""
     from .params import flat_of
     fe = _f_encoder(model)
-    input_ids, img_feat = batch["input_ids"], batch.get("v_feat")
-    fplan, dev, pos_keys = fe._plan_for(input_ids, img_feat, batch["attn_masks"],
-                                        batch.get("gather_index"), batch.get(PLAN_KEY))
-    y = fe.encode_packed(fplan, dev, input_ids, batch.get("position_ids"), img_feat,
-                         batch.get("f_pos_ids"), pos_keys=pos_keys, out_f32=True)
     labels = batch["txt_labels"]
     n = int(labels.shape[0])
     if n == 0:
         return 0
-    tgt = batch["txt_mask_tgt"].to(y.device, non_blocking=True)
-    flat_idx = torch.nonzero_static(tgt.reshape(-1), size=n).reshape(-1)
-    tok = dev.f_pad_to_tok.long()[flat_idx]
-    head = fe.lm_head
-    h = head.LayerNorm(gelu(head.dense(y[tok].to(head.dense.weight.dtype))))
+    h = fe.mlm_head_input(batch["input_ids"], batch.get("position_ids"), batch.get("v_feat"),
+                          batch.get("f_pos_ids"), batch["attn_masks"], batch.get("gather_index"),
+                          batch["txt_mask_tgt"], n, batch.get(PLAN_KEY))
     emb = fe.embeddings.word_embeddings.weight
     ops.lm_head_ce_stats(h.to(torch.bfloat16).contiguous(), flat_of(fe, h.device).bf16(emb),
-                         head.bias.detach().float().contiguous(),
+                         fe.lm_head.bias.detach().float().contiguous(),
                          labels.to(device=h.device, dtype=torch.int32), emb.shape[0] - fe.vocab_pad,
                          acc=acc)
     return n

@@ -226,16 +226,60 @@ def transformer_stack(x, cfg, params, x_f32=None):
     return _TransformerStack.apply(x, x_f32, cfg, *params)
 
 
-def _slot_table_grad(dx, off, idx, slot_pos, dtable, tok_pos):
-    """dtable[pos] += sum of dx rows that used position `pos`. Rows are grouped per slot with a
-    CSR gather-sum; `slot_pos` maps slot -> table row (None: fall back to a per-token index_add)."""
-    if slot_pos is None:
-        dtable.index_add_(0, tok_pos.long(), dx.float())
-        return
-    n_slot = off.numel() - 1
-    dslot = torch.zeros((n_slot, dx.shape[1]), dtype=F32, device=dx.device)
-    ops.gather_sum_rows(dx, off, idx, dslot)
-    dtable.index_add_(0, slot_pos[:n_slot].long(), dslot)
+# Embedding segments shared by the embedding Functions below. Each writes its LayerNorm output
+# into the packed rows `tok` of (emb, emb32) with dropout `d`, drawn by the caller (the order of
+# DropoutState.next() draws fixes the masks). The position table's gradient is a CSR gather-sum
+# straight into its rows (`pos_off / pos_idx`: plan.table_csr over the position ids read).
+def _txt_seg_fwd(tabs, n, tok, ids, pos_ids, d, emb, emb32):
+    """Text tokens: LN(word[id] + pos[p] + type[1]) (model/embed.py:44-58).
+    tabs = (word, pos, type, ln_w, ln_b). Returns what `_txt_seg_bwd` needs."""
+    word, pos, typ, ln_w, ln_b = tabs
+    mean, rstd = torch.empty(n, device=emb.device), torch.empty(n, device=emb.device)
+    ops.ln_fwd(word, ln_w, ln_b, 1e-5, emb, n_rows=n, x_rows=ids, add_tab=pos, add_idx=pos_ids,
+               add_vec=typ[1], y_rows=tok, mean=mean, rstd=rstd, drop=d, y_f32=emb32)
+    return mean, rstd, d
+
+
+def _txt_seg_bwd(demb, tabs, st, n, tok, ids, pos_ids, pos_off, pos_idx, pad_idx, dtyp):
+    """Gradients of `_txt_seg_fwd` into the word, position and LayerNorm parameters, and the type
+    row into `dtyp[1]`. Returns autograd's values for (word, pos, ln_w, ln_b)."""
+    word, pos, typ, ln_w, ln_b = tabs
+    mean, rstd, d = st
+    dword, r_word = _sink(word)
+    dpos, r_pos = _sink(pos)
+    dlnw, r_lnw = _sink(ln_w)
+    dlnb, r_lnb = _sink(ln_b)
+    dx = torch.empty((n, word.shape[1]), dtype=BF16, device=demb.device)
+    ops.ln_bwd(demb, word, ln_w, mean, rstd, n_rows=n, x_rows=ids, add_tab=pos, add_idx=pos_ids,
+               add_vec=typ[1], y_rows=tok, drop=d, dx=dx, d_x_tab=dword, x_pad_idx=pad_idx,
+               dgamma=dlnw, dbeta=dlnb)
+    ops.gather_sum_rows(dx, pos_off, pos_idx, dpos[:pos_off.numel() - 1])
+    ops.colsum(dx, dtyp[1])
+    return r_word, r_pos, r_lnw, r_lnb
+
+
+def _frame_seg_fwd(g, tabs, n, t, tok, d, emb, emb32):
+    """Frames: LN(g + pos[t]) (model/embed.py:146-161); tok None: row i of g -> row i.
+    tabs = (pos, ln_w, ln_b)."""
+    pos, ln_w, ln_b = tabs
+    mean, rstd = torch.empty(n, device=g.device), torch.empty(n, device=g.device)
+    ops.ln_fwd(g, ln_w, ln_b, 1e-5, emb, n_rows=n, add_tab=pos, add_idx=t, y_rows=tok, mean=mean,
+               rstd=rstd, drop=d, y_f32=emb32)
+    return mean, rstd, d
+
+
+def _frame_seg_bwd(demb, g, tabs, st, n, t, tok, pos_off, pos_idx):
+    """Returns (d g, autograd's values for (pos, ln_w, ln_b))."""
+    pos, ln_w, ln_b = tabs
+    mean, rstd, d = st
+    dg = torch.empty((n, g.shape[1]), dtype=BF16, device=g.device)
+    dlnw, r_lnw = _sink(ln_w)
+    dlnb, r_lnb = _sink(ln_b)
+    ops.ln_bwd(demb, g, ln_w, mean, rstd, n_rows=n, add_tab=pos, add_idx=t, y_rows=tok, drop=d,
+               dx=dg, dgamma=dlnw, dbeta=dlnb)
+    dpos, r_pos = _sink(pos)
+    ops.gather_sum_rows(dg, pos_off, pos_idx, dpos[:pos_off.numel() - 1])
+    return dg, (r_pos, r_lnw, r_lnb)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -246,23 +290,17 @@ class _CrossModalEmbed(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, cfg, *params):
-        word, pos, typ, ln_w, ln_b = params[:5]
+        word, typ = params[0], params[2]
         drop = cfg["drop"]
         n_tok, H = cfg["n_tok"], word.shape[1]
         emb = torch.empty((n_tok, H), dtype=BF16, device=word.device)
         emb32 = torch.empty((n_tok, H), dtype=F32, device=word.device)   # residual of layer 0
         type_row = typ[1]
         st = {}
-        # text tokens: LN(word[id] + pos[pid] + type[1]) -> packed row  (model/embed.py:44-58)
         n_txt = cfg["n_txt"]
         if n_txt:
-            st["t_mean"] = torch.empty(n_txt, device=word.device)
-            st["t_rstd"] = torch.empty(n_txt, device=word.device)
-            st["t_drop"] = drop.next(drop.hidden_p)
-            ops.ln_fwd(word, ln_w, ln_b, 1e-5, emb, n_rows=n_txt, x_rows=cfg["txt_ids"],
-                       add_tab=pos, add_idx=cfg["txt_pos"], add_vec=type_row,
-                       y_rows=cfg["txt_tok"], mean=st["t_mean"], rstd=st["t_rstd"],
-                       drop=st["t_drop"], y_f32=emb32)
+            st["t"] = _txt_seg_fwd(params[:5], n_txt, cfg["txt_tok"], cfg["txt_ids"],
+                                   cfg["txt_pos"], drop.next(drop.hidden_p), emb, emb32)
         n_img = cfg["n_img"]
         if n_img:
             (lin_w, lin_b, iln_w, iln_b, ipos, mask_emb, oln_w, oln_b) = params[5:13]
@@ -280,7 +318,7 @@ class _CrossModalEmbed(torch.autograd.Function):
             st["o_rstd"] = torch.empty(n_img, device=word.device)
             st["o_drop"] = drop.next(drop.hidden_p)
             ops.ln_fwd(proj, oln_w, oln_b, 1e-5, emb, n_rows=n_img, add_tab=ipos,
-                       add_idx=cfg["img_k"], add_vec=type_row, y_rows=cfg["img_tok"],
+                       add_idx=cfg["img_pos"], add_vec=type_row, y_rows=cfg["img_tok"],
                        mean=st["o_mean"], rstd=st["o_rstd"], drop=st["o_drop"], y_f32=emb32)
             st["xn"], st["proj"] = xn, proj
         ctx.cfg, ctx.st = cfg, st
@@ -294,7 +332,7 @@ class _CrossModalEmbed(torch.autograd.Function):
             EXCHANGE_HOOK[0].embedding_backward_begins()
         cfg, st = ctx.cfg, ctx.st
         params = ctx.params
-        word, pos, typ, ln_w, ln_b = params[:5]
+        word, typ = params[0], params[2]
         demb = demb.contiguous()
         H = word.shape[1]
         dev = word.device
@@ -303,20 +341,9 @@ class _CrossModalEmbed(torch.autograd.Function):
         n_txt, n_img = cfg["n_txt"], cfg["n_img"]
         type_row = typ[1]
         if n_txt:
-            dword, grads[0] = _sink(word)
-            dpos, grads[1] = _sink(pos)
-            dlnw, grads[3] = _sink(ln_w)
-            dlnb, grads[4] = _sink(ln_b)
-            dx = torch.empty((n_txt, H), dtype=BF16, device=dev)
-            ops.ln_bwd(demb, word, ln_w, st["t_mean"], st["t_rstd"], n_rows=n_txt,
-                       x_rows=cfg["txt_ids"], add_tab=pos, add_idx=cfg["txt_pos"],
-                       add_vec=type_row, y_rows=cfg["txt_tok"], drop=st["t_drop"], dx=dx,
-                       d_x_tab=dword, x_pad_idx=cfg["pad_idx"], dgamma=dlnw, dbeta=dlnb)
-            # position rows are shared by every sequence: deterministic CSR gather-sum per
-            # text slot, then slot -> position id (identity for the collate's arange ids)
-            _slot_table_grad(dx, cfg["txtpos_off"], cfg["txtpos_idx"], cfg["txt_slot_pos"], dpos,
-                             cfg.get("txt_pos"))
-            ops.colsum(dx, dtyp[1])
+            grads[0], grads[1], grads[3], grads[4] = _txt_seg_bwd(
+                demb, params[:5], st["t"], n_txt, cfg["txt_tok"], cfg["txt_ids"], cfg["txt_pos"],
+                cfg["txtpos_off"], cfg["txtpos_idx"], cfg["pad_idx"], dtyp)
         if n_img:
             (lin_w, lin_b, iln_w, iln_b, ipos, mask_emb, oln_w, oln_b) = params[5:13]
             D = iln_w.numel()
@@ -324,12 +351,12 @@ class _CrossModalEmbed(torch.autograd.Function):
             doln_w, grads[11] = _sink(oln_w)
             doln_b, grads[12] = _sink(oln_b)
             ops.ln_bwd(demb, st["proj"], oln_w, st["o_mean"], st["o_rstd"], n_rows=n_img,
-                       add_tab=ipos, add_idx=cfg["img_k"], add_vec=type_row,
+                       add_tab=ipos, add_idx=cfg["img_pos"], add_vec=type_row,
                        y_rows=cfg["img_tok"], drop=st["o_drop"], dx=dproj, dgamma=doln_w,
                        dbeta=doln_b)
             dipos, grads[9] = _sink(ipos)
-            _slot_table_grad(dproj, cfg["imgpos_off"], cfg["imgpos_idx"], cfg["img_slot_pos"],
-                             dipos, cfg.get("img_k"))
+            ops.gather_sum_rows(dproj, cfg["imgpos_off"], cfg["imgpos_idx"],
+                                dipos[:cfg["imgpos_off"].numel() - 1])
             ops.colsum(dproj, dtyp[1])
             dlin_b, grads[6] = _sink(lin_b)
             ops.colsum(dproj, dlin_b)
@@ -428,14 +455,11 @@ class _FrameEmbed(torch.autograd.Function):
     @staticmethod
     def forward(ctx, g, cfg, pos, ln_w, ln_b):
         drop = cfg["drop"]
-        n, H = g.shape
         z = torch.empty_like(g)
         z32 = torch.empty(g.shape, dtype=F32, device=g.device)    # residual of layer 0
-        mean, rstd = torch.empty(n, device=g.device), torch.empty(n, device=g.device)
-        d = drop.next(drop.hidden_p)
-        ops.ln_fwd(g, ln_w, ln_b, 1e-5, z, n_rows=n, add_tab=pos, add_idx=cfg["t"], mean=mean,
-                   rstd=rstd, drop=d, y_f32=z32)
-        ctx.cfg, ctx.st = cfg, (mean, rstd, d)
+        ctx.st = _frame_seg_fwd(g, (pos, ln_w, ln_b), g.shape[0], cfg["t"], None,
+                                drop.next(drop.hidden_p), z, z32)
+        ctx.cfg = cfg
         ctx.save_for_backward(g)
         ctx.params = (pos, ln_w, ln_b)
         ctx.mark_non_differentiable(z32)
@@ -444,20 +468,10 @@ class _FrameEmbed(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dz, _dz32=None):
         cfg = ctx.cfg
-        mean, rstd, d = ctx.st
         (g,) = ctx.saved_tensors
-        pos, ln_w, ln_b = ctx.params
-        dz = dz.contiguous()
-        n, H = dz.shape
-        dgx = torch.empty_like(dz)
-        dln_w, r_ln_w = _sink(ln_w)
-        dln_b, r_ln_b = _sink(ln_b)
-        ops.ln_bwd(dz, g, ln_w, mean, rstd, n_rows=n, add_tab=pos, add_idx=cfg["t"], drop=d,
-                   dx=dgx, dgamma=dln_w, dbeta=dln_b)
-        dpos, r_pos = _sink(pos)
-        n_slot = cfg["pos_off"].numel() - 1
-        ops.gather_sum_rows(dgx, cfg["pos_off"], cfg["pos_idx"], dpos[:n_slot])
-        return dgx, None, r_pos, r_ln_w, r_ln_b
+        dg, grads = _frame_seg_bwd(dz.contiguous(), g, ctx.params, ctx.st, g.shape[0], cfg["t"],
+                                   None, cfg["pos_off"], cfg["pos_idx"])
+        return (dg, None) + grads
 
 
 def frame_embed(g, cfg, params):
@@ -476,24 +490,19 @@ class _QaFusedEmbed(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, g, cfg, *params):
-        c_pos, c_ln_w, c_ln_b, word, f_pos, typ, f_ln_w, f_ln_b = params
         drop, dev = cfg["drop"], g.device
         n_tok, n_frm, n_qa = cfg["n_tok"], cfg["n_frm"], cfg["n_qa"]
         H = g.shape[1]
         emb = torch.empty((n_tok, H), dtype=BF16, device=dev)
         emb32 = torch.empty((n_tok, H), dtype=F32, device=dev)
-        st = {"f_mean": torch.empty(n_frm, device=dev), "f_rstd": torch.empty(n_frm, device=dev),
-              "q_mean": torch.empty(n_qa, device=dev), "q_rstd": torch.empty(n_qa, device=dev),
-              "f_drop": drop.next(cfg["frm_p"]), "q_drop": drop.next(cfg["qa_p"])}
+        d_frm, d_qa = drop.next(cfg["frm_p"]), drop.next(cfg["qa_p"])
+        st = {}
         if n_frm:
-            ops.ln_fwd(g, c_ln_w, c_ln_b, 1e-5, emb, n_rows=n_frm, add_tab=c_pos,
-                       add_idx=cfg["frm_t"], y_rows=cfg["frm_tok"], mean=st["f_mean"],
-                       rstd=st["f_rstd"], drop=st["f_drop"], y_f32=emb32)
+            st["f"] = _frame_seg_fwd(g, params[:3], n_frm, cfg["frm_t"], cfg["frm_tok"], d_frm,
+                                     emb, emb32)
         if n_qa:
-            ops.ln_fwd(word, f_ln_w, f_ln_b, 1e-5, emb, n_rows=n_qa, x_rows=cfg["qa_ids"],
-                       add_tab=f_pos, add_idx=cfg["qa_pos"], add_vec=typ[1],
-                       y_rows=cfg["qa_tok"], mean=st["q_mean"], rstd=st["q_rstd"],
-                       drop=st["q_drop"], y_f32=emb32)
+            st["q"] = _txt_seg_fwd(params[3:], n_qa, cfg["qa_tok"], cfg["qa_ids"], cfg["qa_pos"],
+                                   d_qa, emb, emb32)
         ctx.cfg, ctx.st, ctx.params = cfg, st, params
         ctx.save_for_backward(g)
         ctx.mark_non_differentiable(emb32)
@@ -501,37 +510,20 @@ class _QaFusedEmbed(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, demb, _demb32=None):
-        cfg, st = ctx.cfg, ctx.st
-        c_pos, c_ln_w, c_ln_b, word, f_pos, typ, f_ln_w, f_ln_b = ctx.params
+        cfg, st, params = ctx.cfg, ctx.st, ctx.params
         (g,) = ctx.saved_tensors
         demb = demb.contiguous()
         n_frm, n_qa = cfg["n_frm"], cfg["n_qa"]
-        H = g.shape[1]
         grads = [None] * 8
-        dg = torch.empty((n_frm, H), dtype=BF16, device=g.device)
+        dg = torch.empty((n_frm, g.shape[1]), dtype=BF16, device=g.device)
         if n_frm:
-            dlnw, grads[1] = _sink(c_ln_w)
-            dlnb, grads[2] = _sink(c_ln_b)
-            ops.ln_bwd(demb, g, c_ln_w, st["f_mean"], st["f_rstd"], n_rows=n_frm, add_tab=c_pos,
-                       add_idx=cfg["frm_t"], y_rows=cfg["frm_tok"], drop=st["f_drop"], dx=dg,
-                       dgamma=dlnw, dbeta=dlnb)
-            dpos, grads[0] = _sink(c_pos)
-            n_slot = cfg["cpos_off"].numel() - 1
-            ops.gather_sum_rows(dg, cfg["cpos_off"], cfg["cpos_idx"], dpos[:n_slot])
+            dg, grads[0:3] = _frame_seg_bwd(demb, g, params[:3], st["f"], n_frm, cfg["frm_t"],
+                                            cfg["frm_tok"], cfg["cpos_off"], cfg["cpos_idx"])
         if n_qa:
-            dword, grads[3] = _sink(word)
-            dlnw, grads[6] = _sink(f_ln_w)
-            dlnb, grads[7] = _sink(f_ln_b)
-            dx = torch.empty((n_qa, H), dtype=BF16, device=g.device)
-            ops.ln_bwd(demb, word, f_ln_w, st["q_mean"], st["q_rstd"], n_rows=n_qa,
-                       x_rows=cfg["qa_ids"], add_tab=f_pos, add_idx=cfg["qa_pos"], add_vec=typ[1],
-                       y_rows=cfg["qa_tok"], drop=st["q_drop"], dx=dx, d_x_tab=dword,
-                       x_pad_idx=cfg["pad_idx"], dgamma=dlnw, dbeta=dlnb)
-            dpos, grads[4] = _sink(f_pos)
-            n_slot = cfg["qpos_off"].numel() - 1
-            ops.gather_sum_rows(dx, cfg["qpos_off"], cfg["qpos_idx"], dpos[:n_slot])
-            dtyp, grads[5] = _sink(typ)
-            ops.colsum(dx, dtyp[1])
+            dtyp, grads[5] = _sink(params[5])
+            grads[3], grads[4], grads[6], grads[7] = _txt_seg_bwd(
+                demb, params[3:], st["q"], n_qa, cfg["qa_tok"], cfg["qa_ids"], cfg["qa_pos"],
+                cfg["qpos_off"], cfg["qpos_idx"], cfg["pad_idx"], dtyp)
         ctx.st = None
         return (dg, None) + tuple(grads)
 

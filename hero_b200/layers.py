@@ -199,7 +199,7 @@ class BertEncoder(nn.Module):
         N, L, H = hidden_states.shape
         if attention_mask is None:
             attention_mask = torch.ones(N, L, dtype=torch.long, device=hidden_states.device)
-        plan = TxtPlan(attention_mask, with_embedding=False)
+        plan = TxtPlan(attention_mask)
         dev = plan.to(hidden_states.device)
         flat_in = hidden_states.reshape(N * L, H)
         x32 = Fn.gather_rows(flat_in.float(), dev.f_tok_flat, dev.f_pad_to_tok)

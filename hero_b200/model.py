@@ -22,7 +22,7 @@ from .encoder import (CrossModalTrm, RobertaModelConfig, RobertaPreTrainedModel,
                       load_pretrained_weight)
 from .layers import GELU, BertLayerNorm, LinearLayer, MLPLayer
 from .params import flat_of
-from .plan import PLAN_KEY, JointPlan, ReprPlan, TxtPlan
+from .plan import PLAN_KEY, JointPlan, ReprPlan, TxtPlan, plan_inputs
 
 BF16 = torch.bfloat16
 
@@ -118,7 +118,7 @@ class HierarchicalVlModel(VideoPreTrainedModel):
     def _plan(self, batch):
         plan = batch[PLAN_KEY]
         if plan is None:
-            plan = ReprPlan(batch)      # reads the masks back to the host once (one sync)
+            plan = ReprPlan(plan_inputs(batch))   # reads masks and ids back in one copy
         return plan
 
     def repr_packed(self, batch, plan, encode_clip=True, txt_batch=None, txt_plan=None):
@@ -131,19 +131,19 @@ class HierarchicalVlModel(VideoPreTrainedModel):
         fe, ce = self.f_encoder, self.c_encoder
         drop = fe.encoder.dropout_state()
         yq = None
+        shared = batch["c_v_feats"] if batch["f_v_feats"] is None else None
         if txt_batch is None:
             # cross-modal transformer on packed [frames, text] rows
-            hf = fe.encode_packed(plan.f, dev, batch["f_sub_input_ids"], batch["f_sub_pos_ids"],
-                                  batch["f_v_feats"], batch["f_v_pos_ids"], batch["f_v_masks"],
-                                  drop, shared_feats=batch["c_v_feats"]
-                                  if batch["f_v_feats"] is None else None)
+            hf = fe.encode_packed(plan.f, dev, plan.f.seq.attn(dev, "f_"), batch["f_v_feats"],
+                                  batch["f_v_masks"], drop, shared_feats=shared)
         else:
             jplan = plan.__dict__.get("_joint")
             if jplan is None or jplan.t is not txt_plan:
                 jplan = JointPlan(plan, txt_plan)
                 plan.__dict__["_joint"] = jplan
-            y = fe.encode_packed_joint(jplan, dev, txt_plan.to(device), jplan.to(device), batch,
-                                       txt_batch, drop)
+            jdev = jplan.to(device)
+            y = fe.encode_packed(jplan, jdev, jplan.attn(jdev), batch["f_v_feats"],
+                                 batch["f_v_masks"], drop, shared_feats=shared)
             hf, yq = y[:jplan.n_video_tok], y[jplan.n_video_tok:]
         # frame outputs back onto the clip timeline + projected raw features (residual)
         c_v = batch["c_v_feats"]
@@ -189,7 +189,7 @@ class HierarchicalVlModel(VideoPreTrainedModel):
         plan = self._plan(batch)
         tplan = txt_batch.get(PLAN_KEY) if hasattr(txt_batch, "get") else None
         if tplan is None:
-            tplan = TxtPlan(txt_batch["attn_masks"])
+            tplan = TxtPlan(**plan_inputs(txt_batch, "txt"))
         y, dev, yq = self.repr_packed(batch, plan, encode_clip, txt_batch, tplan)
         clip = self._unpack_c(y, dev, plan.shape_c)
         tdev = tplan.to(y.device)

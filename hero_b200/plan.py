@@ -42,12 +42,27 @@ def _max_vl_of(batch):
     return int(batch["f_v_pos_ids"].shape[-1])
 
 
-def _host_ids(t):
-    """Small id tensor -> host int64 array [rows, L], or None if absent / not on the host."""
-    if t is None or (torch.is_tensor(t) and t.device.type != "cpu"):
-        return None
+def _rows(t):
+    """Id array -> int64 [rows, L] (a 1-D array is one row)."""
     a = np.asarray(_np(t), np.int64)
     return a.reshape(1, -1) if a.ndim == 1 else a
+
+
+def _host_arrays(ts):
+    """Tensors, arrays or None -> numpy arrays or None. Tensors that live on a device come back
+    in ONE device->host copy."""
+    on_dev = [t for t in ts if torch.is_tensor(t) and t.device.type != "cpu"]
+    if not on_dev:
+        return [None if t is None else _np(t) for t in ts]
+    flat = torch.cat([t.reshape(-1).to(torch.int64) for t in on_dev]).cpu().numpy()
+    out, o = [], 0
+    for t in ts:
+        if torch.is_tensor(t) and t.device.type != "cpu":
+            out.append(flat[o:o + t.numel()].reshape(tuple(t.shape)))
+            o += t.numel()
+        else:
+            out.append(None if t is None else _np(t))
+    return out
 
 
 class DeviceIndex:
@@ -187,7 +202,7 @@ class FPlan:
         else:
             gi = _np(gather_index).astype(np.int64)
             src = gi[s.tok_row, s.tok_col]
-            self.max_sl = int(max_sl)
+            self.max_sl = int(max_sl or 0)
         self.max_vl = int(max_vl)
         is_img = src < self.max_vl
         tok = np.arange(s.n_tok, dtype=np.int32)
@@ -201,34 +216,37 @@ class FPlan:
                         + self.txt_j).astype(np.int32)                  # index in input_ids.view(-1)
         self.n_img = int(self.img_tok.size)
         self.n_txt = int(self.txt_tok.size)
+        self.n_tok = s.n_tok
 
     def arrays(self, prefix="f_"):
+        """The attention plan under `prefix`, and the embedding arrays (`embed_ids`) unprefixed."""
         a = self.seq.arrays(prefix)
-        a.update({prefix + "img_tok": self.img_tok, prefix + "img_k": self.img_k,
-                  prefix + "img_src": self.img_src, prefix + "txt_tok": self.txt_tok,
-                  prefix + "txt_j": self.txt_j, prefix + "txt_src": self.txt_src})
-        for name in ("txt_ids", "txt_pos", "img_kpos"):
-            v = getattr(self, name, None)
-            if v is not None:
-                a[prefix + name] = v
+        a.update(getattr(self, "emb", {}))
         return a
 
-    def gather_ids(self, input_ids=None, pos_ids=None, img_pos_ids=None):
-        """Per packed token: its vocabulary id, text position id and frame position id, gathered
-        HERE on the host (collate side) when the id tensors are host tensors, so the forward
-        does not spend ~15 small index kernels on them. All optional: what is missing is gathered
-        on the device as before."""
-        ids, pos, ipos = _host_ids(input_ids), _host_ids(pos_ids), _host_ids(img_pos_ids)
-        self.txt_ids = self.txt_pos = self.img_kpos = None
-        if ids is not None and self.n_txt:
-            self.txt_ids = ids.reshape(-1)[self.txt_src].astype(np.int32)
-        if pos is not None and self.n_txt:
-            if pos.shape[0] == 1:
-                self.txt_pos = pos[0][self.txt_j].astype(np.int32)
-            elif ids is not None and pos.shape == ids.shape:
-                self.txt_pos = pos.reshape(-1)[self.txt_src].astype(np.int32)
-        if ipos is not None and self.n_img:
-            self.img_kpos = ipos.reshape(-1)[self.img_k].astype(np.int32)
+    def embed_ids(self, input_ids=None, pos_ids=None, img_pos_ids=None, padding_idx=1):
+        """The index arrays of functional.cross_modal_embed (`self.emb`), gathered here on the
+        host: per packed text token its row (txt_tok), vocabulary id and position id; per packed
+        frame token its row, feature row (img_src) and position id; and for each position table a
+        CSR over the position ids the tokens read (deterministic table gradients). Missing
+        `pos_ids` follow SubEmbeddings.create_position_ids_from_input_ids; missing `img_pos_ids`
+        are the frame slots."""
+        txt_ids = txt_pos = np.zeros(0, np.int64)
+        if self.n_txt:
+            ids = _rows(input_ids)
+            if pos_ids is None:
+                keep = ids != padding_idx
+                pos = np.cumsum(keep, 1) * keep + padding_idx
+            else:
+                pos = _rows(pos_ids)
+            txt_ids = ids.reshape(-1)[self.txt_src]
+            txt_pos = pos[0][self.txt_j] if pos.shape[0] == 1 else pos.reshape(-1)[self.txt_src]
+        img_pos = self.img_k if img_pos_ids is None else \
+            _rows(img_pos_ids).reshape(-1)[self.img_k]
+        self.emb = {"txt_tok": self.txt_tok, "txt_ids": txt_ids.astype(np.int32),
+                    "img_tok": self.img_tok, "img_src": self.img_src}
+        self.emb.update(pos_csr("txt", txt_pos))
+        self.emb.update(pos_csr("img", img_pos))
 
 
 class CPlan:
@@ -284,8 +302,16 @@ def table_csr(idx, n_rows):
     return _csr(idx, np.arange(idx.size, dtype=np.int32), n_rows)
 
 
+def pos_csr(name, pos):
+    """`{name}_pos` (per-token position ids, int32) and the `table_csr` over them,
+    `{name}pos_off / idx`, covering the table rows up to the largest id used."""
+    pos = np.asarray(pos, np.int32)
+    off, idx = table_csr(pos, int(pos.max()) + 1 if pos.size else 1)
+    return {name + "_pos": pos, name + "pos_off": off, name + "pos_idx": idx}
+
+
 class ReprPlan:
-    """Everything HierarchicalVlModel.forward_repr needs for one batch."""
+    """Everything HierarchicalVlModel.forward_repr needs for one batch (a `plan_inputs` dict)."""
 
     def __init__(self, batch):
         # `plan_inputs` dicts carry the two padded lengths instead of the big tensors
@@ -305,49 +331,40 @@ class ReprPlan:
         self.f.shared_feats_ok = self.shared_feats_ok = bool((self.f.img_src_c >= 0).all())
         self.shape_f = tuple(batch["f_attn_masks"].shape)
         self.shape_c = tuple(batch["c_attn_masks"].shape)
-        # position-table CSRs for the deterministic embedding gradients
-        self.f_txtpos_off, self.f_txtpos_idx = table_csr(self.f.txt_j, max(max_sl, 1))
-        self.f_imgpos_off, self.f_imgpos_idx = table_csr(self.f.img_k, max(max_vl, 1))
+        # position-table CSR of the temporal embeddings
         self.c_pos_off, self.c_pos_idx = table_csr(self.c.c_t, max(self.shape_c[1], 1))
-        # subtitle position ids as the collate made them (lets JointPlan decide on the host
-        # whether video and query rows share one slot -> position table)
         get = batch.get if hasattr(batch, "get") else (lambda k: None)
-        self.sub_pos = _host_ids(get("f_sub_pos_ids"))
-        self.f.gather_ids(get("f_sub_input_ids"), get("f_sub_pos_ids"), get("f_v_pos_ids"))
+        self.f.embed_ids(get("f_sub_input_ids"), get("f_sub_pos_ids"), get("f_v_pos_ids"))
+        self.f.emb["img_src_c"] = self.f.img_src_c
         self.dev = None
 
     def to(self, device, staging=None):
         if self.dev is None or self.dev.flat.device != torch.device(device):
             a = self.f.arrays("f_")
-            a["f_img_src_c"] = self.f.img_src_c
             a.update(self.c.arrays("c_"))
-            a.update({"f_txtpos_off": self.f_txtpos_off, "f_txtpos_idx": self.f_txtpos_idx,
-                      "f_imgpos_off": self.f_imgpos_off, "f_imgpos_idx": self.f_imgpos_idx,
-                      "c_pos_off": self.c_pos_off, "c_pos_idx": self.c_pos_idx})
+            a.update({"c_pos_off": self.c_pos_off, "c_pos_idx": self.c_pos_idx})
             self.dev = DeviceIndex(a, torch.device(device), staging)
         return self.dev
 
 
 class TxtPlan:
-    """Text-only rows (CrossModalTrm 'txt' task, and the generic BertEncoder API)."""
+    """Rows of a CrossModalTrm pass without the clip level: text-only rows (the 'txt' task; with
+    no `input_ids`, the generic BertEncoder API, which needs no embedding arrays) or, with
+    `gather_index`, the frame + text rows of an MLM batch (data/mlm.py mlm_collate). Built from
+    `plan_inputs(batch, "txt")` or `plan_inputs(batch, "mlm")`."""
 
-    def __init__(self, attn_mask, with_embedding=True, pos_ids=None, input_ids=None):
-        self.f = FPlan(attn_mask)
+    def __init__(self, attn_mask, input_ids=None, pos_ids=None, gather_index=None,
+                 img_pos_ids=None, max_vl=0):
+        max_sl = None if input_ids is None else input_ids.shape[1]
+        self.f = FPlan(attn_mask, gather_index, max_vl, max_sl)
         self.shape = tuple(_np(attn_mask).shape)
-        self.with_embedding = with_embedding
-        self.pos = _host_ids(pos_ids)
-        if with_embedding:
-            self.f.gather_ids(input_ids, pos_ids)
-        if with_embedding:
-            self.pos_off, self.pos_idx = table_csr(self.f.txt_j, max(self.shape[1], 1))
+        if input_ids is not None or self.f.n_txt == 0:
+            self.f.embed_ids(input_ids, pos_ids, img_pos_ids)
         self.dev = None
 
     def to(self, device, staging=None):
         if self.dev is None or self.dev.flat.device != torch.device(device):
-            a = self.f.arrays("f_")
-            if self.with_embedding:
-                a.update({"pos_off": self.pos_off, "pos_idx": self.pos_idx})
-            self.dev = DeviceIndex(a, torch.device(device), staging)
+            self.dev = DeviceIndex(self.f.arrays("f_"), torch.device(device), staging)
         return self.dev
 
 
@@ -365,7 +382,7 @@ class JointPlan:
         self.n_tok = a + fq.seq.n_tok
         self.n_txt = fv.n_txt + fq.n_txt
         self.n_img = fv.n_img
-        self.max_vl, self.max_sl_v, self.max_sl_q = fv.max_vl, fv.max_sl, fq.max_sl
+        self.shared_feats_ok = rplan.shared_feats_ok
         sv, sq = fv.seq, fq.seq
         self.n_seq = sv.n_seq + sq.n_seq
         self.max_len = max(sv.max_len, sq.max_len)
@@ -373,6 +390,10 @@ class JointPlan:
         # long-sequence tiles (rare) of both row kinds go last, after every 128-token tile
         self.n_long = sv.n_long + sq.n_long
         self.max_long = max(sv.max_long, sq.max_long)
+        if not hasattr(fq, "emb"):
+            raise ValueError("the query plan was built without input_ids: build it with "
+                             "TxtPlan(**plan_inputs(batch, 'txt'))")
+        ev, eq = fv.emb, fq.emb
         self.arr = {
             "j_cu": np.concatenate([sv.cu, sq.cu[1:] + a]).astype(np.int32),
             "j_seq_lo": np.concatenate([sv.seq_lo, sq.seq_lo + a]).astype(np.int32),
@@ -381,24 +402,11 @@ class JointPlan:
                                            sq.long_tok0 + a]).astype(np.int32),
             "j_tile_ntok": np.concatenate([sv.short_ntok, sq.short_ntok, sv.long_ntok,
                                            sq.long_ntok]).astype(np.int32),
-            "j_txt_tok": np.concatenate([fv.txt_tok, fq.txt_tok + a]).astype(np.int32),
-            "j_txt_j": np.concatenate([fv.txt_j, fq.txt_j]).astype(np.int32),
+            "txt_tok": np.concatenate([ev["txt_tok"], eq["txt_tok"] + a]).astype(np.int32),
+            "txt_ids": np.concatenate([ev["txt_ids"], eq["txt_ids"]]).astype(np.int32),
         }
-        n_slot = max(fv.max_sl, fq.max_sl, 1)
-        self.arr["j_txtpos_off"], self.arr["j_txtpos_idx"] = table_csr(self.arr["j_txt_j"], n_slot)
-        for name in ("txt_ids", "txt_pos"):      # host-gathered ids of both row kinds, if known
-            a_v, a_q = getattr(fv, name, None), getattr(fq, name, None)
-            if (a_v is not None or fv.n_txt == 0) and a_q is not None:
-                parts = ([a_v] if fv.n_txt else []) + [a_q]
-                self.arr["j_" + name] = np.concatenate(parts).astype(np.int32)
-        # Do both row kinds use the same slot -> position map (the collate's arange)? Decided here
-        # on the host when the plans saw the position ids; None = unknown (the encoder then has
-        # to compare the device tensors, which costs a device sync per step).
-        self.same_slot_pos = None
-        pv, pq = getattr(rplan, "sub_pos", None), getattr(tplan, "pos", None)
-        if pv is not None and pq is not None and pv.shape[0] == 1 and pq.shape[0] == 1:
-            n = min(pv.shape[1], pq.shape[1])
-            self.same_slot_pos = bool(np.array_equal(pv[0, :n], pq[0, :n]))
+        self.arr.update(pos_csr("txt", np.concatenate([ev["txt_pos"], eq["txt_pos"]])))
+        self.arr.update({k: v for k, v in ev.items() if k.startswith("img")})
         self.dev = None
 
     def to(self, device, staging=None):
@@ -478,27 +486,47 @@ class QaPlan:
 
 PLAN_KEY = "_hero_plan"
 QA_PLAN_KEY = "_hero_qa_plan"
-_REPR_KEYS = ("f_attn_masks", "f_gather_index", "c_attn_masks", "num_subs", "sub_idx2frame_idx")
+QUERY_PLAN_KEY = "_hero_query_plan"
+_REPR_KEYS = ("f_attn_masks", "f_gather_index", "c_attn_masks", "f_sub_input_ids",
+              "f_sub_pos_ids", "f_v_pos_ids")
+# TxtPlan arguments and the batch keys they come from, per kind
+_TXT_ARGS = ("attn_mask", "input_ids", "pos_ids", "gather_index", "img_pos_ids")
+_TXT_KEYS = {"txt": ("attn_masks", "input_ids", "pos_ids", None, None),
+             "mlm": ("attn_masks", "input_ids", "position_ids", "gather_index", "f_pos_ids")}
+# key prefix of the query-fused text of each kind: question + answer rows of video QA, the
+# statement rows of VIOLIN
+_QA_PREFIX = {"videoqa": "qa", "violin": "q"}
+_QA_ARGS = ("qa_attn_masks", "qa_input_ids", "qa_pos_ids")
+
+
+def _qa_keys(prefix):
+    return tuple(prefix + k[2:] for k in _QA_ARGS)
 
 
 def plan_inputs(batch, kind="repr"):
-    """The small, picklable part of a host batch that a plan is built from (masks and index
-    lists as numpy arrays; none of the feature tensors) — what is shipped to a PlanPool worker."""
-    def opt(key):
-        v = batch.get(key) if hasattr(batch, "get") else None
-        return None if v is None else _np(v)
-
-    if kind not in ("repr",) + tuple(_QA_PREFIX):
-        return {"attn_masks": _np(batch["attn_masks"]), "pos_ids": opt("pos_ids"),
-                "input_ids": opt("input_ids")}
-    d = {k: (_np(batch[k]) if torch.is_tensor(batch[k]) else batch[k]) for k in _REPR_KEYS}
-    if kind in _QA_PREFIX:
-        d["_qa"] = qa_plan_inputs(batch, _QA_PREFIX[kind])
-    d["f_sub_pos_ids"] = opt("f_sub_pos_ids")
-    d["f_sub_input_ids"] = opt("f_sub_input_ids")
-    d["f_v_pos_ids"] = opt("f_v_pos_ids")
+    """The small, picklable part of a batch that a plan is built from: masks and id tensors as
+    host arrays, index lists and padded lengths; none of the feature tensors. Every plan is built
+    from it, in collate workers, PlanPool processes or, without an attached plan, in the forward;
+    tensors that live on the device come back in ONE device->host copy.
+    kind: 'repr' (video batch), 'videoqa' / 'violin' (+ the QaPlan arguments under "_qa"),
+    'txt' (query batch) or 'mlm' (data/mlm.py batch): the last two give TxtPlan's arguments."""
+    get = batch.get if hasattr(batch, "get") else batch.__getitem__
+    if kind in _TXT_KEYS:
+        keys = _TXT_KEYS[kind]
+        d = dict(zip(_TXT_ARGS, _host_arrays([None if k is None else get(k) for k in keys])))
+        if d["gather_index"] is not None:
+            d["max_vl"] = int(batch["v_feat"].shape[1])
+        return d
+    keys = _REPR_KEYS + (_qa_keys(_QA_PREFIX[kind]) if kind in _QA_PREFIX else ())
+    d = dict(zip(keys, _host_arrays([get(k) for k in keys])))
+    for k in ("num_subs", "sub_idx2frame_idx"):
+        d[k] = _np(batch[k]) if torch.is_tensor(batch[k]) else batch[k]
     d["_max_vl"] = _max_vl_of(batch)
     d["_max_sl"] = int(batch["f_sub_input_ids"].shape[1])
+    if kind in _QA_PREFIX:
+        qa = [d.pop(k) for k in keys[len(_REPR_KEYS):]]
+        d["_qa"] = dict(zip(_QA_ARGS, qa), c_attn_masks=d["c_attn_masks"],
+                        n_videos=int(batch["targets"].shape[0]))
     return d
 
 
@@ -511,8 +539,7 @@ def build_plans(repr_in, txt_in=None):
         rplan.__dict__["_qa"] = QaPlan(**repr_in["_qa"])
     if txt_in is None:
         return rplan, None
-    tplan = TxtPlan(txt_in["attn_masks"], pos_ids=txt_in.get("pos_ids"),
-                    input_ids=txt_in.get("input_ids"))
+    tplan = TxtPlan(**txt_in)
     rplan.__dict__["_joint"] = JointPlan(rplan, tplan)
     return rplan, tplan
 
@@ -547,43 +574,31 @@ class PlanPool:
         self._ex.shutdown(wait=False, cancel_futures=True)
 
 
-QUERY_PLAN_KEY = "_hero_query_plan"
-
-
 def attach_plan(batch, kind="repr"):
     """Collate-side hook: build the plan from HOST tensors (no device sync later) and stash it in
     the batch dict; `move_to_cuda`-style helpers leave non-tensor values alone.
-    kind: 'repr' (video batch), 'txt' (query batch), 'vsm' — a VSM / VCMR training batch that
-    carries its queries as `query_input_ids / query_pos_ids / query_attn_masks` (data/vcmr.py):
-    attaches the video plan, the query plan (QUERY_PLAN_KEY) and their joint plan — or 'videoqa'
-    (data/videoQA.py video_qa_collate) / 'violin' (data/violin.py violin_collate): the video plan
-    of the cross-modal rows and the QaPlan of the query-fused temporal rows (QA_PLAN_KEY).
-    The plan captures the batch's token / position ids per packed token (FPlan.gather_ids): attach
+    kind: 'repr' (video batch), 'txt' (query batch), 'mlm' (data/mlm.py batch), 'vsm' — a VSM /
+    VCMR training batch that carries its queries as `query_input_ids / query_pos_ids /
+    query_attn_masks` (data/vcmr.py): attaches the video plan, the query plan (QUERY_PLAN_KEY) and
+    their joint plan — or 'videoqa' (data/videoQA.py video_qa_collate) / 'violin'
+    (data/violin.py violin_collate): the video plan of the cross-modal rows and the QaPlan of the
+    query-fused temporal rows (QA_PLAN_KEY).
+    The plan captures the batch's token / position ids per packed token (FPlan.embed_ids): attach
     it AFTER any masking of `input_ids` (the reference masks in the dataset, before collate), and
     attach again if the ids are edited afterwards."""
+    if kind in _TXT_KEYS:
+        batch[PLAN_KEY] = TxtPlan(**plan_inputs(batch, kind))
+        return batch
+    query = None
     if kind == "vsm":
-        rplan = ReprPlan(batch)
-        tplan = TxtPlan(batch["query_attn_masks"], pos_ids=batch.get("query_pos_ids"),
-                        input_ids=batch.get("query_input_ids"))
-        rplan.__dict__["_joint"] = JointPlan(rplan, tplan)
-        batch[PLAN_KEY], batch[QUERY_PLAN_KEY] = rplan, tplan
-        return batch
-    if kind in _QA_PREFIX:
-        batch[PLAN_KEY] = ReprPlan(batch)
-        batch[QA_PLAN_KEY] = qa_plan(batch, _QA_PREFIX[kind])
-        return batch
-    if kind == "repr":
-        batch[PLAN_KEY] = ReprPlan(batch)
-    else:
-        get = batch.get if hasattr(batch, "get") else (lambda k: None)
-        batch[PLAN_KEY] = TxtPlan(batch["attn_masks"], pos_ids=get("pos_ids"),
-                                  input_ids=get("input_ids"))
+        query = plan_inputs({k: batch.get("query_" + k) for k in _TXT_KEYS["txt"][:3]}, "txt")
+    rplan, tplan = build_plans(plan_inputs(batch, "repr" if kind == "vsm" else kind), query)
+    batch[PLAN_KEY] = rplan
+    if tplan is not None:
+        batch[QUERY_PLAN_KEY] = tplan
+    if "_qa" in rplan.__dict__:
+        batch[QA_PLAN_KEY] = rplan.__dict__.pop("_qa")
     return batch
-
-
-# key prefix of the query-fused text of each kind: question + answer rows of video QA, the
-# statement rows of VIOLIN
-_QA_PREFIX = {"videoqa": "qa", "violin": "q"}
 
 
 def video_kind(batch):
@@ -596,28 +611,10 @@ def video_kind(batch):
     return "repr"
 
 
-def qa_plan_inputs(batch, prefix="qa"):
-    """QaPlan arguments of a batch whose query-fused text is `{prefix}_attn_masks / _input_ids /
-    _pos_ids`, as host arrays. `targets` gives the number of videos: (Nv, 1) in video QA, one row
-    per statement in VIOLIN. Tensors that live on the device come back in ONE device->host copy."""
-    ts = [batch[k] for k in ("c_attn_masks", f"{prefix}_attn_masks", f"{prefix}_input_ids",
-                             f"{prefix}_pos_ids")]
-    dev = next((t.device for t in ts if torch.is_tensor(t) and t.device.type != "cpu"), None)
-    if dev is None:
-        arrays = [_np(t) for t in ts]
-    else:
-        parts = [torch.as_tensor(t).to(dev).reshape(-1).to(torch.int64) for t in ts]
-        flat = torch.cat(parts).cpu().numpy()
-        offs = np.cumsum([0] + [p.numel() for p in parts])
-        arrays = [flat[o:e].reshape(tuple(t.shape)) for o, e, t in zip(offs[:-1], offs[1:], ts)]
-    d = dict(zip(("c_attn_masks", "qa_attn_masks", "qa_input_ids", "qa_pos_ids"), arrays))
-    d["n_videos"] = int(batch["targets"].shape[0])
-    return d
-
-
 def qa_plan(batch, prefix="qa"):
     """QaPlan of a video_qa_collate batch (prefix "qa") or a violin_collate batch ("q")."""
-    return QaPlan(**qa_plan_inputs(batch, prefix))
+    keys = ("c_attn_masks",) + _qa_keys(prefix)
+    return QaPlan(*_host_arrays([batch[k] for k in keys]), int(batch["targets"].shape[0]))
 
 
 class TvcPlan:

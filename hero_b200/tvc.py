@@ -31,7 +31,7 @@ from . import ops
 from .layers import BertIntermediate, BertLayerNorm, BertOutput, BertSelfAttention, BertSelfOutput
 from .model import HeroModel
 from .params import flat_of
-from .plan import PLAN_KEY, ReprPlan, TvcPlan
+from .plan import PLAN_KEY, ReprPlan, TvcPlan, plan_inputs
 
 BF16 = torch.bfloat16
 MAX_DECODE_STEP = 1023      # position table of 1024 entries (hero_tvc.json d_config)
@@ -148,12 +148,12 @@ class HeroForTvc(HeroModel):
         """model/tvc.py:219-238 without the padding: (packed clip-level outputs fp32
         [n_c_tokens, H] of HierarchicalVlModel.repr_packed, TvcPlan of the caption segments). Uses
         the ReprPlan attached with plan.attach_plan, else builds it (one device->host read of the
-        masks)."""
+        masks and ids)."""
         if not isinstance(batch, defaultdict):
             batch = defaultdict(lambda: None, batch)
         rplan = batch[PLAN_KEY]
         if rplan is None:
-            rplan = ReprPlan(batch)
+            rplan = ReprPlan(plan_inputs(batch))
         tplan = TvcPlan(batch["clip_ranges"], rplan)
         flat_of(self, batch["c_v_feats"].device)   # one flat buffer for encoder and decoder
         y, _ = self.v_encoder.repr_packed(batch, rplan)

@@ -24,22 +24,21 @@ from torch.nn import functional as F
 from . import functional as Fn
 from .layers import MLPLayer, mask_logits
 from .model import HeroModel
-from .plan import PLAN_KEY, QA_PLAN_KEY, ReprPlan, qa_plan
+from .plan import PLAN_KEY, QA_PLAN_KEY, build_plans, plan_inputs, video_kind
 
 TASKS = ("tvqa", "how2qa")
 
 
-def encode_query_fused(model, batch, prefix="qa"):
+def encode_query_fused(model, batch):
     """Packed fp32 temporal-transformer outputs of every query-fused row (model/videoQA.py:64-82,
     model/violin.py:53-67), with the batch's QaPlan and its device index. The query text is
-    `{prefix}_input_ids / _pos_ids / _attn_masks`. Plans attached to the batch
-    (plan.attach_plan) are used; otherwise they are built here from the masks and query ids (one
+    `qa_input_ids / _pos_ids / _attn_masks` (video QA) or `q_...` (VIOLIN). Plans attached to the
+    batch (plan.attach_plan) are used; otherwise they are built here from the masks and ids (one
     host read)."""
     rplan, qplan = batch[PLAN_KEY], batch[QA_PLAN_KEY]
-    if rplan is None:
-        rplan = ReprPlan(batch)
-    if qplan is None:
-        qplan = qa_plan(batch, prefix)
+    if rplan is None or qplan is None:
+        built, _ = build_plans(plan_inputs(batch, video_kind(batch)))
+        rplan, qplan = rplan or built, qplan or built.__dict__.pop("_qa")
     ve = model.v_encoder
     g, _ = ve.repr_packed(batch, rplan, encode_clip=False)
     dev = qplan.to(g.device)

@@ -36,7 +36,7 @@ class HeroForViolin(HeroModel):
         batch = defaultdict(lambda: None, batch)
         if task != "violin":
             raise ValueError(f"Unrecognized task: {task}")
-        y, qplan, dev = encode_query_fused(self, batch, prefix="q")
+        y, qplan, dev = encode_query_fused(self, batch)
         rows, length = qplan.n_videos, qplan.length
         video_masks = batch["c_attn_masks"].float()
         pooled = Fn.qa_pool(y, self.violin_pool.weight, None, dev.frame_map, video_masks, rows, 1,

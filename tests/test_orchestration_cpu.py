@@ -102,6 +102,8 @@ def test_generic_bert_encoder_and_temporal_apis(tmp_path, monkeypatch):
 
 
 def test_plan_can_be_attached_at_collate_time(tmp_path, monkeypatch):
+    """Plans attached at collate time give the outputs of the plans the forward builds itself,
+    separately and in the fused joint pass."""
     fake_ops.install(monkeypatch)
     from hero_b200.plan import PLAN_KEY, attach_plan
     fx = gu.load("hier_tiny.npz")
@@ -115,34 +117,37 @@ def test_plan_can_be_attached_at_collate_time(tmp_path, monkeypatch):
         qa = model.f_encoder(qb, "txt")[0]
         qb2 = attach_plan(dict(qb), kind="txt")
         qb_out = model.f_encoder(qb2, "txt")[0]
+        ja, jqa = model.forward_repr_txt(dict(vb), dict(qb))
+        jb, jqb = model.forward_repr_txt(vb2, qb2)
     assert torch.equal(a, b)
     assert torch.equal(qa, qb_out)
-
-
-def test_host_gathered_ids_equal_the_device_gathers(tmp_path, monkeypatch):
-    """Plans built from host id tensors carry the per-token vocabulary / position ids
-    (FPlan.gather_ids); plans built without them (ids already on the device) leave the gathers
-    to the forward. Both must give the same outputs, separately and in the fused joint pass."""
-    fake_ops.install(monkeypatch)
-    from hero_b200 import plan as hp
-    fx = gu.load("hier_tiny.npz")
-    model = _model(tmp_path, fx)
-    vb, qb = gu.stored_batches(fx)
-    with torch.no_grad():
-        vb1, qb1 = hp.attach_plan(dict(vb)), hp.attach_plan(dict(qb), kind="txt")
-        assert vb1[hp.PLAN_KEY].f.txt_ids is not None and qb1[hp.PLAN_KEY].f.txt_ids is not None
-        a, qa = model(vb1, "repr"), model.f_encoder(qb1, "txt")[0]
-        ja, jqa = model.forward_repr_txt(dict(vb), dict(qb))
-
-        def no_ids(self, *a, **k):
-            self.txt_ids = self.txt_pos = self.img_kpos = None
-        monkeypatch.setattr(hp.FPlan, "gather_ids", no_ids)
-        vb2, qb2 = hp.attach_plan(dict(vb)), hp.attach_plan(dict(qb), kind="txt")
-        assert vb2[hp.PLAN_KEY].f.txt_ids is None
-        b, qb_out = model(vb2, "repr"), model.f_encoder(qb2, "txt")[0]
-        jb, jqb = model.forward_repr_txt(dict(vb), dict(qb))
-    assert torch.equal(a, b) and torch.equal(qa, qb_out)
     assert torch.equal(ja, jb) and torch.equal(jqa, jqb)
+
+
+def test_per_row_position_ids_give_the_shared_row_results(tmp_path, monkeypatch):
+    """Position ids given per row (R, L) instead of once (1, L) read the same table rows: outputs
+    and every gradient, the position table's included, are the same, plan attached or not."""
+    fake_ops.install(monkeypatch)
+    from hero_b200.plan import attach_plan
+    fx = gu.load("hier_tiny.npz")
+    vb, _ = gu.stored_batches(fx)
+    w1 = torch.from_numpy(fx["loss_w1"])
+    rows = dict(vb, f_sub_pos_ids=vb["f_sub_pos_ids"].expand_as(vb["f_sub_input_ids"]).clone())
+    assert vb["f_sub_pos_ids"].shape[0] == 1 < rows["f_sub_pos_ids"].shape[0]
+
+    def run(batch):
+        model = _model(tmp_path, fx)
+        clip = model(batch, "repr")
+        (clip * w1).sum().backward()
+        return clip.detach(), {k: p.grad for k, p in model.named_parameters()
+                               if p.grad is not None}
+
+    a, ga = run(vb)
+    for batch in (rows, attach_plan(dict(rows))):
+        b, gb = run(batch)
+        assert torch.equal(a, b) and ga.keys() == gb.keys()
+        for k in ga:
+            assert torch.equal(ga[k], gb[k]), k
 
 
 def test_in_place_gradient_sinks_match_autograd_accumulation(tmp_path, monkeypatch):

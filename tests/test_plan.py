@@ -1,10 +1,11 @@
 """Host-side packing plans (pure numpy): checked against the padded-layout semantics of the
 reference as restated by the oracle (gather of cat[img, txt]; collect_frame_outputs)."""
 import numpy as np
+import pytest
 import torch
 
 from hero_b200 import synth
-from hero_b200.plan import FPlan, ReprPlan, SeqPlan, TxtPlan, table_csr
+from hero_b200.plan import FPlan, ReprPlan, SeqPlan, TxtPlan, plan_inputs
 from oracle import hero_oracle as orc
 
 
@@ -77,16 +78,34 @@ def test_duplicate_frame_assignments_accumulate():
     assert counts.tolist() == [1, 1, 2, 1, 0, 0]
 
 
+def _check_pos_csr(e, name, n):
+    """The position-table CSR lists every packed token once, under the position id it reads."""
+    pos, off, idx = e[name + "_pos"], e[name + "pos_off"], e[name + "pos_idx"]
+    assert off[-1] == n == pos.size and np.array_equal(np.sort(idx), np.arange(n))
+    for p in range(len(off) - 1):
+        assert (pos[idx[off[p]:off[p + 1]]] == p).all()
+
+
 def test_txt_plan_and_table_csr():
     _, qb = _ragged()
-    tp = TxtPlan(qb["attn_masks"])
-    assert tp.f.n_img == 0 and tp.f.n_txt == int(qb["attn_masks"].sum())
+    tp = TxtPlan(**plan_inputs(qb, "txt"))
+    valid = qb["attn_masks"].bool().numpy()
+    assert tp.f.n_img == 0 and tp.f.n_txt == int(valid.sum())
     ids = qb["input_ids"].view(-1).numpy()[tp.f.txt_src]
-    assert np.array_equal(ids, qb["input_ids"].numpy()[qb["attn_masks"].bool().numpy()])
-    off, idx = table_csr(tp.f.txt_j, qb["attn_masks"].shape[1])
-    for j in range(len(off) - 1):
-        assert all(tp.f.txt_j[t] == j for t in idx[off[j]:off[j + 1]])
-    assert off[-1] == tp.f.n_txt
+    assert np.array_equal(ids, qb["input_ids"].numpy()[valid])
+    e = tp.f.emb
+    assert np.array_equal(e["txt_ids"], ids)
+    pos = np.broadcast_to(qb["pos_ids"].numpy(), valid.shape)[valid]
+    assert np.array_equal(e["txt_pos"], pos)
+    _check_pos_csr(e, "txt", tp.f.n_txt)
+    # without position ids: SubEmbeddings.create_position_ids_from_input_ids, on the host
+    from types import SimpleNamespace
+    from hero_b200.embed import SubEmbeddings
+    tp2 = TxtPlan(**dict(plan_inputs(qb, "txt"), pos_ids=None))
+    want = SubEmbeddings.create_position_ids_from_input_ids(SimpleNamespace(padding_idx=1),
+                                                            qb["input_ids"])
+    assert np.array_equal(tp2.f.emb["txt_pos"], want.numpy()[valid])
+    _check_pos_csr(tp2.f.emb, "txt", tp2.f.n_txt)
 
 
 def test_dense_canonical_batch_shapes():
@@ -171,12 +190,13 @@ def test_frame_slots_map_back_to_clip_frames():
     assert np.array_equal(plan2.f.img_src_c, plan.f.img_src_c)
 
 
-def test_plan_invariants_on_random_batches():
+def test_plan_invariants_and_position_csrs_on_random_batches():
     """Property test (hypothesis): for random ragged batches — including subtitles without frames,
     frames matched by no subtitle or by several, single-token rows — the plan is a bijection
     between packed tokens and valid padded positions, attention tiles partition the token stream
-    without splitting a sequence, the two frame-merge CSRs are transposes of each other, and the
-    joint (video + query) plan is the concatenation of its parts."""
+    without splitting a sequence, the two frame-merge CSRs are transposes of each other, the
+    joint (video + query) plan is the concatenation of its parts, and every position-table CSR
+    lists each token under the position id it reads."""
     from hypothesis import given, settings, strategies as st
     from hero_b200.plan import ATTN_TILE, JointPlan
 
@@ -186,7 +206,7 @@ def test_plan_invariants_on_random_batches():
         vb, qb = synth.syn_tvr_ragged(batch_size=bs, seed=seed, vfeat_dim=8, vocab=60,
                                       t_range=(3, 40), s_range=(1, 6), l_range=(1, 9),
                                       q_range=(1, 8))
-        rp, tp = ReprPlan(vb), TxtPlan(qb["attn_masks"], pos_ids=qb["pos_ids"])
+        rp, tp = ReprPlan(vb), TxtPlan(**plan_inputs(qb, "txt"))
         for sp, mask in ((rp.f.seq, vb["f_attn_masks"]), (rp.c.seq, vb["c_attn_masks"]),
                          (tp.f.seq, qb["attn_masks"])):
             valid = np.flatnonzero(mask.numpy().reshape(-1))
@@ -208,7 +228,14 @@ def test_plan_invariants_on_random_batches():
         a = rp.f.seq.n_tok
         assert jp.n_tok == a + tp.f.seq.n_tok and jp.n_tiles == rp.f.seq.n_tiles + tp.f.seq.n_tiles
         assert np.array_equal(jp.arr["j_seq_lo"][a:], tp.f.seq.seq_lo + a)
-        assert jp.same_slot_pos in (True, False)
+        for e, n in ((rp.f.emb, rp.f.n_txt), (tp.f.emb, tp.f.n_txt), (jp.arr, jp.n_txt)):
+            _check_pos_csr(e, "txt", n)
+        _check_pos_csr(rp.f.emb, "img", rp.f.n_img)
+        assert np.array_equal(jp.arr["txt_pos"], np.concatenate([rp.f.emb["txt_pos"],
+                                                                 tp.f.emb["txt_pos"]]))
+        # a query plan without token ids cannot feed the joint embedding
+        with pytest.raises(ValueError, match="input_ids"):
+            JointPlan(rp, TxtPlan(qb["attn_masks"], pos_ids=qb["pos_ids"]))
 
     check()
 
