@@ -7,6 +7,8 @@ Semantics kept from the reference (SURVEY.md Appendix D.8):
     result is mean-over-ranks / denom (utils/distributed.py:19-46).
   * `broadcast_tensors(tensors, root)` (utils/distributed.py:103-151), `all_gather_list`,
     `any_broadcast` (utils/distributed.py:182-212).
+  * `sum_over_ranks`: the evaluation merge of device sums (the reference sums host values from
+    `all_gather_list`), in a fixed rank order so every rank holds the same bits.
   * `VsmAllgather`: forward all-gather, backward = own slice of the incoming gradient with no
     reduction (model/pretrain.py:427-447).
 What changes is the mechanism: when the gradients already live in one flat buffer
@@ -257,6 +259,27 @@ def all_gather_list(data):
     out = [None] * size()
     dist.all_gather_object(out, data)
     return out
+
+
+def sum_over_ranks(t):
+    """Sum over ranks of a small fp32 / fp64 tensor (metric sums and counts), on its device and
+    without a host synchronisation: one all_gather_into_tensor into a (W, n) buffer, then the rows
+    added in rank order. The order of the additions is fixed, so the result is bitwise the same on
+    every rank; all_reduce(SUM) would leave it to NCCL's algorithm. Returns a new tensor of t's
+    shape (a copy of t without a process group). Host data goes through `all_gather_list`."""
+    if t.dtype not in (torch.float32, torch.float64):
+        raise TypeError(f"sum_over_ranks takes fp32 / fp64 tensors, not {t.dtype}")
+    flat = t.detach().reshape(-1).contiguous()
+    if not dist.is_initialized():
+        return flat.clone().view(t.shape)
+    world = dist.get_world_size()
+    rows = torch.empty(world * flat.numel(), dtype=t.dtype, device=t.device)
+    dist.all_gather_into_tensor(rows, flat)
+    rows = rows.view(world, flat.numel())
+    out = rows[0].clone()
+    for r in range(1, world):
+        out += rows[r]
+    return out.view(t.shape)
 
 
 def any_broadcast(data, root_rank):

@@ -15,15 +15,23 @@
   temporal NMS of the ranked lists on the device (csrc/nms.cu), carried home in the same copy, and
   the TVR recall metrics of utils/tvr_standalone_eval.py vectorised over queries on the host
   (DESIGN §4 "Temporal NMS and TVR metrics").
-* `validate_videoqa` — eval_videoQA.py:120-173 for one process on HeroForVideoQA.
-* `validate_violin` — eval_violin.py:118-164 for one process on HeroForViolin.
+* `validate_videoqa` — eval_videoQA.py:120-173 on HeroForVideoQA.
+* `validate_violin` — eval_violin.py:118-164 on HeroForViolin.
 * `validate_pretrain` (and `validate_mlm` / `_mffr` / `_mfm_nce` / `_fom` / `_vsm`) —
-  pretrain.py:387-608 for one process: the fused LM-head GEMM with `hero_ce_finish_stats` for MLM
-  and MFM-NCE (no logits tensor), `hero_row_l2_cos` for l2 / cosine, sums on the device, one
-  device->host copy per task (DESIGN §4 "Pretraining validation").
+  pretrain.py:387-608: the fused LM-head GEMM with `hero_ce_finish_stats` for MLM and MFM-NCE (no
+  logits tensor), `hero_row_l2_cos` for l2 / cosine, sums on the device, one device->host copy per
+  task (DESIGN §4 "Pretraining validation").
+* `decode_tvc` — greedy TVC captions of inf_tvc.py / train_tvc.py.
 * `ModelSaver` / `TrainingRestorer` — utils/save.py:112-181 with the same file layout (`vocab_padded`
   flag, `model_step_<n>.pt`, `train_state_<n>.pt`, `restore.pt` + backup), so checkpoints are
   interchangeable with the reference's; optimizer state is FusedAdamW's flat moments.
+
+Data-parallel evaluation (DESIGN §4 "Data-parallel evaluation"): when `distributed.size() > 1`,
+every evaluation entry point above evaluates what its own rank was given (its loader's batches,
+its corpus clips, its query batches and their ground truth) and returns the result merged over all
+ranks, the same on every rank. Device sums go through `distributed.sum_over_ranks`, host records
+and dicts through `distributed.all_gather_list`. Without a process group, or with one rank,
+nothing is exchanged.
 """
 import os
 from collections import OrderedDict
@@ -32,9 +40,15 @@ from os.path import exists, join
 import numpy as np
 import torch
 
-from . import ops
+from . import distributed, ops
 from .loader import BatchStager
 from .plan import PLAN_KEY, attach_plan
+
+
+def _data_parallel():
+    """True when the evaluation is sharded: each rank evaluates the batches it was given and every
+    entry point returns the result merged over all ranks."""
+    return distributed.size() > 1
 
 
 @torch.no_grad()
@@ -43,7 +57,14 @@ def embed_video_corpus(model, batches, n_videos, max_clip_len, device=None, vide
     """`batches`: iterable of HOST video batch dicts (reference `video_collate` layout; plans are
     attached here when the collate has not). `video_indices`: per batch the row of each clip in the
     corpus tensors (default: consecutive). Returns (frame_embeddings (n_videos, max_clip_len', H),
-    c_attn_masks (n_videos, max_clip_len')) trimmed to the longest clip seen, like the reference."""
+    c_attn_masks (n_videos, max_clip_len')) trimmed to the longest clip seen, like the reference.
+
+    Data-parallel (`distributed.size() > 1`), each rank embeds the clips of its own `batches` at
+    their global rows, and every rank returns the whole corpus: the rows of all ranks must cover
+    0..n_videos-1 exactly once (checked on the gathered host indices before any collective,
+    ValueError otherwise), the trim is to the longest clip of any rank, and the zero-initialised
+    corpus and masks are summed over ranks (each row has one writer, so the sum is exact). A rank
+    without clips still joins; its corpus is allocated with the model's hidden size."""
     v_enc = model.v_encoder if hasattr(model, "v_encoder") else model
     device = device or next(v_enc.parameters()).device
     was_training = v_enc.training
@@ -51,6 +72,8 @@ def embed_video_corpus(model, batches, n_videos, max_clip_len, device=None, vide
     stager = BatchStager(device, depth=3)
     cur = torch.cuda.current_stream(device)
     total, masks, longest, row = None, None, 0, 0
+    sharded = _data_parallel()
+    claimed = []                                         # host rows of this rank's clips
     it = iter(batches)
 
     def stage_next():
@@ -76,19 +99,61 @@ def embed_video_corpus(model, batches, n_videos, max_clip_len, device=None, vide
             total = torch.zeros((n_videos, max_clip_len, Hd), dtype=out_dtype, device=device)
             masks = torch.zeros((n_videos, max_clip_len), dtype=batch["c_attn_masks"].dtype,
                                 device=device)
+        if sharded:
+            rows = (np.asarray(video_indices[bi], dtype=np.int64).reshape(-1)
+                    if video_indices is not None else np.arange(row, row + B))
+            claimed.append(rows)
+            if rows.size and (rows.min() < 0 or rows.max() >= n_videos):
+                rows = None             # reported by every rank in _merge_corpus, not written
         if video_indices is not None:
             idx = torch.as_tensor(video_indices[bi], device=device, dtype=torch.long)
         else:
             idx = torch.arange(row, row + B, device=device)
-        total[idx, :T] = emb.to(out_dtype)
-        masks[idx, :T] = batch["c_attn_masks"]
+        if not sharded or rows is not None:
+            total[idx, :T] = emb.to(out_dtype)
+            masks[idx, :T] = batch["c_attn_masks"]
         longest = max(longest, T)
         row += B
         bi += 1
     if was_training:
         v_enc.train()
+    if sharded:
+        return _merge_corpus(v_enc, total, masks, longest, claimed, n_videos, max_clip_len,
+                             device, out_dtype)
     if total is None:
         return None, None
+    return total[:, :longest], masks[:, :longest]
+
+
+def _merge_corpus(v_enc, total, masks, longest, claimed, n_videos, max_clip_len, device,
+                  out_dtype):
+    """The data-parallel end of `embed_video_corpus`: one host gather of every rank's rows,
+    longest clip and mask dtype; the row check; then the corpus and masks all-reduced (SUM) and
+    trimmed to the longest clip of any rank."""
+    import torch.distributed as dist
+    mine = np.concatenate(claimed) if claimed else np.zeros(0, dtype=np.int64)
+    parts = distributed.all_gather_list((mine, longest, None if masks is None else masks.dtype))
+    rows = np.concatenate([p[0] for p in parts])
+    inside = rows[(rows >= 0) & (rows < n_videos)]
+    count = np.bincount(inside, minlength=n_videos)
+    outside = np.setdiff1d(rows, inside)
+    twice, missing = np.flatnonzero(count > 1), np.flatnonzero(count == 0)
+    if len(outside) or len(twice) or len(missing):
+        raise ValueError(
+            f"data-parallel corpus of {n_videos} clips: every row must be embedded by exactly one "
+            f"rank; rows outside [0, {n_videos}): {outside[:8].tolist()}, claimed more than once: "
+            f"{twice[:8].tolist()}, claimed by no rank: {missing[:8].tolist()} (first 8 of each)")
+    longest = max(p[1] for p in parts)
+    if longest == 0:
+        return None, None
+    if total is None:
+        mask_dtype = next(p[2] for p in parts if p[2] is not None)
+        hidden = v_enc.config.c_config.hidden_size
+        total = torch.zeros((n_videos, max_clip_len, hidden), dtype=out_dtype, device=device)
+        masks = torch.zeros((n_videos, max_clip_len), dtype=mask_dtype, device=device)
+    # the full buffers, not contiguous copies of the trimmed ones: no second corpus in memory
+    dist.all_reduce(total, op=dist.ReduceOp.SUM)
+    dist.all_reduce(masks, op=dist.ReduceOp.SUM)
     return total[:, :longest], masks[:, :longest]
 
 
@@ -337,7 +402,9 @@ class _QueryStager:
 
 def _run_batches(model, corpus, batches, video_ids, rank_kw, want_gt, post=None):
     """Encodes and ranks every query batch; returns (qids, per-batch host results, has_gt).
-    `post(out)`, when given, maps each batch's device results to the dict that is copied."""
+    `post(out)`, when given, maps each batch's device results to the dict that is copied.
+    Data-parallel, the three are gathered from every rank (all_gather_list) and concatenated in
+    rank order; has_gt holds when it holds on every rank."""
     local = {vid: i for i, vid in enumerate(video_ids)}
     stager = _QueryStager(corpus.device)
     qids_all, results, has_gt = [], [], want_gt
@@ -366,6 +433,11 @@ def _run_batches(model, corpus, batches, video_ids, rank_kw, want_gt, post=None)
         qids_all.extend(qids)
     if was_training:
         model.train()
+    if _data_parallel():        # every rank's queries against the whole corpus, in rank order
+        parts = distributed.all_gather_list((qids_all, results, has_gt))
+        qids_all = [q for p in parts for q in p[0]]
+        results = [r for p in parts for r in p[1]]
+        has_gt = all(p[2] for p in parts)
     return qids_all, results, has_gt
 
 
@@ -410,7 +482,10 @@ def full_vcmr_predictions(model, corpus, batches, video_ids, video2idx, *, tasks
     has a video-level loss weight, and SVMR only when every batch carries its targets. Flat VCMR
     indices are decoded with the corpus's own L (the reference uses max_clip_len; the two agree
     when the corpus holds a clip of max_clip_len frames); see `rank_queries` for the other stated
-    deviations."""
+    deviations.
+
+    Data-parallel, each rank ranks its own query batches against the whole corpus and every rank
+    returns the lists of all ranks' queries, in rank order (eval_vcmr.py:125-134)."""
     tasks = _vcmr_tasks(model, tasks)
     res = {"SVMR": [], "VCMR": [], "VR": []}
     if tasks:
@@ -439,7 +514,8 @@ def full_vcmr_predictions(model, corpus, batches, video_ids, video2idx, *, tasks
 def full_vr_predictions(model, corpus, batches, video_ids, video2idx, *, max_vr_video=100):
     """The ranking half of the reference's full video-retrieval evaluation (eval_vr.py:198-263):
     the top `max_vr_video` clips of every query by its raw video score, the first 100 of them
-    listed as [video_idx, 0, 0, score]. Arguments and result as `full_vcmr_predictions`."""
+    listed as [video_idx, 0, 0, score]. Arguments and result as `full_vcmr_predictions`, also
+    when data-parallel: the lists of every rank's queries, in rank order (eval_vr.py:276-293)."""
     rank_kw = dict(tasks=("VR",), q2c_alpha=None, max_video=max_vr_video)
     qids, results, _ = _run_batches(model, corpus, batches, video_ids, rank_kw, False)
     vr = []
@@ -643,14 +719,40 @@ def _records(qids, vid, st, ed, score, valid):
         for i, (q, c) in enumerate(zip(qids, n))]
 
 
+def _merge_ground_truth(ground_truth):
+    """The ground truth of every rank's queries: each rank's list gathered (all_gather_list) and
+    united in rank order, one entry per desc_id (the first seen), so a rank may pass the ground
+    truth of its own shard, as the reference's partial_query_data is, or of the whole split. None
+    when any rank passes None."""
+    parts = distributed.all_gather_list(ground_truth)
+    if any(p is None for p in parts):
+        return None
+    merged = {}
+    for part in parts:
+        for e in part:
+            merged.setdefault(e["desc_id"], e)
+    return list(merged.values())
+
+
 def full_vcmr_eval(model, corpus, batches, video_ids, video2idx, ground_truth, *,
                    tasks=RANK_TASKS, q2c_alpha=20.0, max_vcmr_video=100, min_pred_l=2,
                    max_pred_l=16, max_before_nms=200, max_after_nms=100, nms_thd=0.5,
                    vfeat_interval=1.5, use_desc_type=True):
     """The reference's full VCMR evaluation from ranking to metrics (validate_full_vcmr,
-    eval_vcmr.py:205-508, one process): rank every query batch, run NMS on the device, copy both
-    lists to the host in the batch's one copy, and score them with `eval_retrieval`'s arithmetic
-    on the packed arrays.
+    eval_vcmr.py:205-508): rank every query batch, run NMS on the device, copy both lists to the
+    host in the batch's one copy, and score them with `eval_retrieval`'s arithmetic on the packed
+    arrays.
+
+    Data-parallel, each rank ranks its own query batches against the whole corpus (see
+    `embed_video_corpus` for the sharded corpus pass), the host arrays of all ranks are gathered in
+    rank order, and every rank builds the same submissions and computes the metrics once over the
+    union. ground_truth is gathered too and united by desc_id: each rank may pass the ground truth
+    of its own queries (the reference's partial_query_data) or that of the whole split; if any
+    rank passes None there are no metrics. Stated deviation: the reference averages each rank's already rounded percentages
+    weighted by its query count (eval_vcmr.py:431-446). The union gives the one-process result
+    whatever the number of ranks: the exact recall rounded to 0.01, where the reference's mean of
+    rounded values lies within 0.005 points of the same exact recall. (The reference weights the
+    "<task>_by_type" entries by the query count too, not by the count of that type.)
 
     Arguments as `full_vcmr_predictions`, plus ground_truth: the GT dicts of the evaluated queries
     (the reference's partial_query_data), or None. Returns {"submission": the top-max_after_nms
@@ -722,6 +824,8 @@ def full_vcmr_eval(model, corpus, batches, video_ids, video2idx, ground_truth, *
         sub["video2idx"] = video2idx
         return sub, packed
 
+    if _data_parallel():
+        ground_truth = _merge_ground_truth(ground_truth)
     with_metrics = has_gt and ground_truth is not None
     iou_thds = (0.5, 0.7)                      # VCMR_IOU_THDS (utils/const.py)
     out = {}
@@ -738,13 +842,18 @@ def full_vcmr_eval(model, corpus, batches, video_ids, video2idx, ground_truth, *
 
 @torch.no_grad()
 def validate_videoqa(model, loader, split, task="tvqa", save_logits=False):
-    """eval_videoQA.py:120-173 (validate_videoQA) for one process: returns (val_log, results,
-    logits) with `valid/loss`, `valid/acc`, `valid/ex_per_s`, results[str(qid)] = predicted answer
-    index and, with `save_logits`, logits[str(qid)] = the candidate logits. Once a batch carries a
-    negative target ("no ground truth") only predictions are made and val_log stays empty, as in
-    the reference. Loss sums and correct counts are computed on the device; each batch makes one
-    device->host copy (answers, loss sum, correct count, smallest target, logits). Averaging across
-    ranks (all_gather_list) is left to the caller. `split` names the split only."""
+    """eval_videoQA.py:120-173 (validate_videoQA): returns (val_log, results, logits) with
+    `valid/loss`, `valid/acc`, `valid/ex_per_s`, results[str(qid)] = predicted answer index and,
+    with `save_logits`, logits[str(qid)] = the candidate logits. Once a batch carries a negative
+    target ("no ground truth") only predictions are made and val_log stays empty, as in the
+    reference. Loss sums and correct counts are computed on the device; each batch makes one
+    device->host copy (answers, loss sum, correct count, smallest target, logits). `split` names
+    the split only.
+
+    Data-parallel, each rank evaluates its own batches; one all_gather_list then sums the loss,
+    the correct count and the example count over ranks, and results / logits are the union of
+    every rank's dicts (eval_videoQA.py:95-99), on every rank. No ground truth on any rank means no
+    val_log on every rank. ex_per_s is the global count over this rank's wall time."""
     import time
     model.eval()
     val_loss, n_ex, tot_score = 0.0, 0, 0
@@ -777,6 +886,9 @@ def validate_videoqa(model, loader, split, task="tvqa", save_logits=False):
             val_loss += b_loss
             tot_score += int(b_correct)
             n_ex += len(qids)
+    if _data_parallel():
+        val_loss, tot_score, n_ex, has_gt_target, results, logits = _merge_qa(
+            val_loss, tot_score, n_ex, has_gt_target, results, logits)
     if has_gt_target:
         tot_time = time.time() - t0
         val_log = {"valid/loss": val_loss / n_ex, "valid/acc": tot_score / n_ex,
@@ -785,15 +897,25 @@ def validate_videoqa(model, loader, split, task="tvqa", save_logits=False):
     return val_log, results, logits
 
 
+def _merge_qa(val_loss, tot_score, n_ex, has_gt, results, logits):
+    """One all_gather_list of a rank's host sums and dicts: the sums added in rank order, the
+    ground-truth flag and-ed, the dicts united."""
+    parts = distributed.all_gather_list((val_loss, tot_score, n_ex, has_gt, results, logits))
+    return (sum(p[0] for p in parts), sum(p[1] for p in parts), sum(p[2] for p in parts),
+            all(p[3] for p in parts), {k: v for p in parts for k, v in p[4].items()},
+            {k: v for p in parts for k, v in p[5].items()})
+
+
 @torch.no_grad()
 def validate_violin(model, loader, split, save_logits=False):
-    """eval_violin.py:118-164 (validate_violin) for one process: returns (val_log, results, logits)
-    with `valid/{split}_loss` (summed binary cross entropy of sigmoid(score) over the examples),
+    """eval_violin.py:118-164 (validate_violin): returns (val_log, results, logits) with
+    `valid/{split}_loss` (summed binary cross entropy of sigmoid(score) over the examples),
     `valid/{split}_acc` and `valid/{split}_ex_per_s`, results[str(qid)] = int(sigmoid(score) > 0.5)
     and, with `save_logits`, logits[str(qid)] = [score]. Predictions, the loss sum and the correct
     count are computed on the device; each batch makes one device->host copy. Unlike the
     reference, a one-row batch works (there `predictions.squeeze().tolist()` is an int and the zip
-    over it raises). Averaging across ranks (all_gather_list) is left to the caller."""
+    over it raises). Data-parallel, the sums and dicts of every rank are merged as in
+    `validate_videoqa` (eval_violin.py:94-98)."""
     import time
     model.eval()
     val_loss, n_ex, tot_score = 0.0, 0, 0
@@ -821,6 +943,9 @@ def validate_violin(model, loader, split, save_logits=False):
         val_loss += float(host[n])
         tot_score += int(host[n + 1])
         n_ex += len(qids)
+    if _data_parallel():
+        val_loss, tot_score, n_ex, _, results, logits = _merge_qa(
+            val_loss, tot_score, n_ex, True, results, logits)
     tot_time = time.time() - t0
     val_log = {f"valid/{split}_loss": val_loss / n_ex, f"valid/{split}_acc": tot_score / n_ex,
                f"valid/{split}_ex_per_s": n_ex / tot_time}
@@ -829,9 +954,24 @@ def validate_violin(model, loader, split, save_logits=False):
 
 
 # ------------------------------------------------------------------ pretraining validation
-# pretrain.py:387-608 for one process. Every metric sum stays in a small fp32 device accumulator;
-# each task makes ONE device->host copy, after its last batch. Example counts come from host-known
-# shapes. Averaging across ranks (all_gather_list) is left to the caller.
+# pretrain.py:387-608. Every metric sum stays in a small fp32 device accumulator; each task makes
+# ONE device->host copy, after its last batch. Example counts come from host-known shapes.
+# Data-parallel, the counts join the sums and the copy reads their sum over ranks (_task_totals).
+def _task_totals(acc, counts):
+    """The one device->host copy of a validation task: its device sums `acc` and its host
+    `counts`, as (list of floats, list of ints). Data-parallel, both go into one fp64 device
+    tensor (counts exact up to 2^53) that `distributed.sum_over_ranks` adds up before the copy:
+    a rank with no batch still joins, and every division uses the global counts."""
+    if not _data_parallel():
+        return acc.cpu().tolist(), list(counts)
+    dev = acc.device
+    both = torch.cat([acc.double()] + [torch.full((1,), float(c), dtype=torch.float64, device=dev)
+                                       for c in counts])
+    host = distributed.sum_over_ranks(both).cpu().tolist()
+    k = acc.numel()
+    return host[:k], [int(c) for c in host[k:]]
+
+
 def attach_mlm_plan(batch):
     """Collate-side hook for MLM batches: plan.attach_plan(batch, "mlm")."""
     return attach_plan(batch, "mlm")
@@ -878,7 +1018,7 @@ def validate_mlm(model, val_loader):
     n_word = 0
     for batch in val_loader:
         n_word += _mlm_batch_stats(model, batch, acc)
-    val_loss, n_correct = acc.cpu().tolist()
+    (val_loss, n_correct), (n_word,) = _task_totals(acc, [n_word])
     tot_time = time.time() - t0
     return {"loss": val_loss / n_word, "acc": n_correct / n_word, "tok_per_s": n_word / tot_time}
 
@@ -899,7 +1039,7 @@ def validate_mffr(model, val_loader):
         if targets.shape[0]:
             ops.row_l2_cos(pred.float().contiguous(), targets.float().contiguous(), acc=acc)
         n_feat += int(targets.shape[0])
-    val_loss, cosine = acc.cpu().tolist()
+    (val_loss, cosine), (n_feat,) = _task_totals(acc, [n_feat])
     tot_time = time.time() - t0
     return {"loss": val_loss / n_feat, "cosine": cosine / n_feat, "feat_per_s": n_feat / tot_time}
 
@@ -937,7 +1077,8 @@ def validate_mfm_nce(model, val_loader):
         if pos.shape[0]:
             _nce_batch_stats(feats, pos, neg_feats, acc_ce, acc_l2)
         n_feat += int(pos.shape[0])
-    val_loss, n_correct, val_l2, cosine = torch.cat([acc_ce, acc_l2]).cpu().tolist()
+    (val_loss, n_correct, val_l2, cosine), (n_feat,) = _task_totals(torch.cat([acc_ce, acc_l2]),
+                                                                    [n_feat])
     tot_time = time.time() - t0
     return {"loss": val_loss / n_feat, "acc": n_correct / n_feat, "l2": val_l2 / n_feat,
             "cosine": cosine / n_feat, "feat_per_s": n_feat / tot_time}
@@ -974,7 +1115,7 @@ def validate_fom(model, val_loader):
         hits = ((scores.argmax(dim=-1) == targets) & valid).sum()
         acc += torch.stack([loss, hits.float(), valid.sum().float()])
         n_ex += len(batch["vids"])
-    val_loss, tot_score, n_valid_ex = acc.cpu().tolist()
+    (val_loss, tot_score, n_valid_ex), (n_ex,) = _task_totals(acc, [n_ex])
     tot_time = time.time() - t0
     return {"valid/loss": val_loss / n_valid_ex, "valid/acc": tot_score / n_valid_ex,
             "valid/ex_per_s": n_ex / tot_time}
@@ -985,8 +1126,18 @@ def validate_vsm(model, val_loader, opts):
     """pretrain.py:409-433: model(batch, 'vsm', compute_loss=True) in eval mode ('sum'
     reductions), the three loss sums accumulated on the device; n_ex = len(q_vidx), the positives
     counted from loss_neg_ctx's shape. Normalised by opts.lw_st_ed / lw_neg_ctx / lw_neg_q as the
-    reference does."""
+    reference does. Data-parallel, the forward takes its in-batch negatives from every rank's
+    current batch (val_gather_gpus, as in the reference), so the ranking losses are those of the
+    gathered batches and every rank must run the same number of VSM batches: the lengths of loaders
+    that have one are compared first, and a difference raises ValueError on every rank (a rank
+    that ran out would otherwise leave the others waiting in the gather)."""
     import time
+    if _data_parallel():
+        lens = distributed.all_gather_list(len(val_loader) if hasattr(val_loader, "__len__")
+                                           else None)
+        if len(set(lens)) > 1:
+            raise ValueError(f"data-parallel VSM validation with {lens} batches on ranks "
+                             f"0..{len(lens) - 1}: every rank must run the same number")
     t0 = time.time()
     acc = torch.zeros(3, dtype=torch.float32, device=_device_of(model))
     use_neg = opts.lw_neg_ctx != 0 or opts.lw_neg_q != 0
@@ -999,7 +1150,8 @@ def validate_vsm(model, val_loader, opts):
             parts += [loss_neg_ctx.sum(), loss_neg_q.sum()]
             n_ex_pos += loss_neg_ctx.numel()
         acc[:len(parts)] += torch.stack(parts).float()
-    val_loss_st_ed, val_loss_neg_ctx, val_loss_neg_q = acc.cpu().tolist()
+    (val_loss_st_ed, val_loss_neg_ctx, val_loss_neg_q), (n_ex, n_ex_pos) = _task_totals(
+        acc, [n_ex, n_ex_pos])
     tot_time = time.time() - t0
     if opts.lw_st_ed:
         val_loss_st_ed /= n_ex
@@ -1017,10 +1169,15 @@ def validate_vsm(model, val_loader, opts):
 
 
 def validate_pretrain(model, val_dataloaders, opts):
-    """pretrain.py:387-406 (validate) for one process: model.eval(), each task's validation
-    chosen by the prefix of its name ('mlm', 'mffr', 'mfm-nce', 'fom', 'vsm'), model.train() on
-    exit. Returns the dict the reference logs, {f'{task}_{k}': v} over all tasks. `opts` needs
-    lw_st_ed, lw_neg_ctx and lw_neg_q. Raises ValueError for an unknown task."""
+    """pretrain.py:387-406 (validate): model.eval(), each task's validation chosen by the prefix
+    of its name ('mlm', 'mffr', 'mfm-nce', 'fom', 'vsm'), model.train() on exit. Returns the dict
+    the reference logs, {f'{task}_{k}': v} over all tasks. `opts` needs lw_st_ed, lw_neg_ctx and
+    lw_neg_q. Raises ValueError for an unknown task.
+
+    Data-parallel, each rank validates the batches of its own loaders and every task's sums and
+    counts are summed over ranks on the device before the task's one copy, as the reference sums
+    them over all_gather_list; every rank returns the same losses and accuracies. The rates
+    (tok_per_s, feat_per_s, ex_per_s) are global counts over this rank's wall time."""
     model.eval()
     out = {}
     try:
@@ -1044,11 +1201,12 @@ def validate_pretrain(model, val_dataloaders, opts):
 
 
 def decode_tvc(model, loader, *, max_step, bos, eos, tokenizer):
-    """inf_tvc.py:83-98 / train_tvc.py:259-283 (decode / validate) for one process: greedy captions
-    of every segment of every batch (tvc.TvcGenerator, one device->host copy per batch) as
+    """inf_tvc.py:83-98 / train_tvc.py:259-283 (decode / validate): greedy captions of every
+    segment of every batch (tvc.TvcGenerator, one device->host copy per batch) as
     `{'vid_name', 'clip_id', 'ts', 'descs': [{'desc': caption}]}` records, in batch order. The
-    tokenizer is any object with `convert_ids_to_tokens` / `convert_tokens_to_string`. Gathering
-    across ranks (all_gather_list) and the COCO caption metrics are left to the caller."""
+    tokenizer is any object with `convert_ids_to_tokens` / `convert_tokens_to_string`.
+    Data-parallel, every rank returns the records of all ranks, gathered with all_gather_list in
+    rank order (train_tvc.py:274). The COCO caption metrics are left to the caller."""
     from .tvc import TvcGenerator
     generator = TvcGenerator(model, max_step, bos, eos, fp16=False)
     model.eval()
@@ -1060,6 +1218,8 @@ def decode_tvc(model, loader, *, max_step, bos, eos, tokenizer):
             output = tokenizer.convert_tokens_to_string(tokenizer.convert_ids_to_tokens(out_ids))
             results.append({"vid_name": vid, "clip_id": cid, "ts": ts,
                             "descs": [{"desc": output}]})
+    if _data_parallel():
+        results = [r for rs in distributed.all_gather_list(results) for r in rs]
     return results
 
 
