@@ -134,6 +134,7 @@ def _declare(lib):
     sig("hero_attn_bwd", vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, f32,
         u32, u32, f32, vp)
     sig("hero_gemm_profile_begin")
+    sig("hero_gemm_set_shared_sms", i32)
     sig("hero_gemm_profile_end", C.POINTER(C.c_double), C.POINTER(C.c_double),
         C.POINTER(C.c_int64))
     sig("hero_bert_stack_fwd", C.POINTER(StackArgs), vp)

@@ -15,6 +15,11 @@ int sm_count();
 // True while hero_gemm_profile_begin/end brackets GEMM launches with timing events (the layer
 // runtime then keeps everything on one stream so per-launch durations do not overlap).
 bool gemm_profile_active();
+// While set (on this host thread), GEMM launches hand out their work items dynamically: the layer
+// runtime's backward, whose dgrad chain and weight-gradient stream share the SMs. A grid that has
+// the SMs to itself keeps the static stride, which measured faster there. Returns the previous
+// setting.
+bool gemm_set_shared_sms(bool on);
 // HERO_SERIAL_PROFILE=1 (development): no programmatic dependent launch and a single stream, so a
 // timeline profiler sees every kernel's own duration (tools/step_profile.py).
 bool serial_profiling();

@@ -21,6 +21,12 @@
 //              waits for the previous one to drain. No CTA-wide barrier in the epilogue.
 // Pipeline: smem full/empty ring (TMA <-> MMA); each stage is consumed by the one WG that owns
 // its tile. The producer runs ahead into the next tile while a consumer runs its epilogue.
+// Work items (tile x k-split): a CTA's first item is blockIdx.x; the next is blockIdx.x +
+// gridDim.x, ... (static), or, for grids that share the SMs with another stream's work
+// (GemmShape::dynamic, the DYN instantiation), claimed by the producer lane from a per-stream device counter as the
+// current item's loads start and passed to the eight consumer warps through a small smem ring
+// (item index, or -1 = no more work). A CTA that reaches an SM late, because a grid on another stream still holds
+// it, then takes fewer items instead of stretching the grid by its full static share.
 //
 // Wide form (BN = 256, the long-K GEMMs): 128 x 256 tiles, cooperative consumers. Both WGs take
 // every tile; WG w issues one wgmma.m64n256k16 per k16 step into rows 64w..64w+63 (again 128
@@ -39,6 +45,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <mutex>
 #include <vector>
 
 #include "common.h"
@@ -60,6 +67,7 @@ constexpr int CONSUMER_REGS = 232;
 constexpr int SLAB_ROWS = 16;                          // rows of a warp's accumulator fragment
 constexpr int SLAB_BYTES = SLAB_ROWS * 128;            // 16 rows x 128 B, swizzle-128B
 constexpr int SMEM_LIMIT = 232448;                     // 227 KB opt-in dynamic shared memory per CTA
+constexpr int SCHED_SLOTS = 4;                         // work-item ring, producer -> consumer warps
 
 // ACT_CE / ACT_CE_GRAD: the LM-head of the MLM task (model/layers.py:330-354 + the cross entropy of
 // model/encoder.py:370-372) without materialising fp32 logits: the forward epilogue reduces every
@@ -79,6 +87,9 @@ struct GemmShape {
   // A_lo B_hi + A_hi B_lo into the same fp32 accumulator (~16 mantissa bits per operand): the
   // frame_transform pre-activation, whose ReLU gate flips on bf16 operand rounding
   int k_passes;
+  // 1: CTAs claim items from the stream's counter (grids that share the SMs with another
+  // stream's work); 0: CTA b takes items b, b + gridDim.x, ... Selects the kernel's DYN form.
+  int dynamic;
 };
 
 struct GemmEpilogue {
@@ -133,6 +144,9 @@ struct GemmCfg {
   static constexpr int SMEM_BYTES = BAR_OFFSET + BAR_BYTES;
   static_assert(STAGES >= 3, "not enough shared memory for a 3-stage pipeline");
   static_assert(SMEM_BYTES <= SMEM_LIMIT, "shared memory budget exceeded");
+  // stage full / empty, residual (one per epilogue warp), work-item full / empty, item indices
+  static_assert((2 * STAGES + NUM_EPI_WARPS + 2 * SCHED_SLOTS) * 8 + SCHED_SLOTS * 4 <= BAR_BYTES,
+                "barrier area too small");
 };
 
 // byte offset of byte `b` of row `r` in a 128-byte-swizzled slab (16-byte unit u stored at u ^ (r & 7))
@@ -140,7 +154,7 @@ __device__ __forceinline__ uint32_t slab_off(int r, int b) {
   return r * 128 + ((((b >> 4) ^ (r & 7))) << 4) + (b & 15);
 }
 
-template <int A_MN, int B_MN, int ACT, int OUT, int RES, int BN>
+template <int A_MN, int B_MN, int ACT, int OUT, int RES, int BN, bool DYN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
                   const __grid_constant__ CUtensorMap tmap_b,
@@ -149,7 +163,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
                   const __grid_constant__ CUtensorMap tmap_res,
                   const __grid_constant__ CUtensorMap tmap_a_lo,
                   const __grid_constant__ CUtensorMap tmap_b_lo, const GemmShape s,
-                  const GemmEpilogue e) {
+                  const GemmEpilogue e, uint32_t* __restrict__ sched) {
   using Cfg = GemmCfg<ACT, OUT, RES, BN>;
   constexpr bool WIDE = (BN == 256);
   constexpr int STAGES = Cfg::STAGES;
@@ -173,6 +187,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
   uint64_t* res_bar = bars + 2 * STAGES;                     // one per epilogue warp
+  uint64_t* item_full = res_bar + NUM_EPI_WARPS;             // work-item ring
+  uint64_t* item_empty = item_full + SCHED_SLOTS;
+  int* item_ring = reinterpret_cast<int*>(item_empty + SCHED_SLOTS);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -188,6 +205,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
       mbar_init(&empty_bar[i], WIDE ? 8 : 4);
     }
     for (int i = 0; i < NUM_EPI_WARPS; ++i) mbar_init(&res_bar[i], 1);
+    for (int i = 0; i < SCHED_SLOTS; ++i) {
+      mbar_init(&item_full[i], 1);
+      mbar_init(&item_empty[i], NUM_EPI_WARPS);   // every consumer warp reads every item
+    }
     fence_barrier_init();
   }
   __syncthreads();
@@ -197,15 +218,28 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
   pdl_launch_dependents();
 
   const int total_tiles = s.num_m_blocks * s.num_n_blocks * s.k_splits;
-  const int first_tile = (int)blockIdx.x;
-  const int tile_step = (int)gridDim.x;
 
   if (warp < 4) {
     // ------------------------------------------------------------- TMA producer
     setmaxnreg_dec<PRODUCER_REGS>();
     if (warp == 0 && lane == 0) {
+      // A CTA's first item is its blockIdx.x; claim c on sched[0] is item gridDim.x + c, and a
+      // claim past the end stops the CTA, so every CTA overshoots exactly once. sched[1] counts
+      // CTAs that have stopped. Both are zero when the grid starts: the previous launch on this
+      // stream left them so, and pdl_wait() above has made its writes visible. The next item is
+      // claimed as the current one starts, so the atomic's round trip hides behind its loads.
+      uint32_t next = blockIdx.x;
       uint32_t it = 0;
-      for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
+      for (uint32_t j = 0;; ++j) {
+        const int tile = next < (uint32_t)total_tiles ? (int)next : -1;
+        if constexpr (DYN) {
+          const uint32_t slot = j % SCHED_SLOTS;
+          mbar_wait(&item_empty[slot], ((j / SCHED_SLOTS) & 1u) ^ 1u);
+          item_ring[slot] = tile;
+          mbar_arrive(&item_full[slot]);
+        }
+        if (tile < 0) break;
+        next = DYN ? gridDim.x + atomicAdd(&sched[0], 1u) : next + gridDim.x;
         const int ks = tile % s.k_splits;
         const int t2 = tile / s.k_splits;
         const int n_blk = t2 % s.num_n_blocks;
@@ -233,6 +267,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
               tma_load_2d(sb, mb, &full_bar[stage], kb * BLOCK_K, n_blk * BN);
           }
         }
+      }
+      // the last CTA to stop claiming returns the counter to zero for the next launch
+      if (DYN) __threadfence();
+      if (DYN && atomicAdd(&sched[1], 1u) == gridDim.x - 1) {
+        __threadfence();
+        sched[0] = 0u;
+        sched[1] = 0u;
       }
     }
   } else {
@@ -265,9 +306,22 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
     uint32_t out_it = 0;
     uint32_t it = 0;   // ring position; advances over the other WG's k-blocks too
     float acc[NHALF][BN / 2];   // ping-pong: rows 0-63, rows 64-127 of the tile; wide: own half
+    // the CTA's j-th work item: by stride, or as the producer claimed it
+    auto next_item = [&](uint32_t j) -> int {
+      if constexpr (!DYN) {
+        const uint32_t t = blockIdx.x + j * gridDim.x;
+        return t < (uint32_t)total_tiles ? (int)t : -1;
+      }
+      const uint32_t slot = j % SCHED_SLOTS;
+      mbar_wait(&item_full[slot], (j / SCHED_SLOTS) & 1u);
+      const int t = *reinterpret_cast<volatile int*>(&item_ring[slot]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&item_empty[slot]);
+      return t;
+    };
 
-    int j = 0;   // local tile index
-    for (int tile = first_tile; tile < total_tiles; tile += tile_step, ++j) {
+    uint32_t j = 0;   // local item index
+    for (int tile = next_item(0); tile >= 0; ++j) {
       const int ks = tile % s.k_splits;
       const int t2 = tile / s.k_splits;
       const int n_blk = t2 % s.num_n_blocks;
@@ -275,8 +329,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
       const int kb0 = ks * s.k_blocks / s.k_splits;
       const int kb1 = (ks + 1) * s.k_blocks / s.k_splits;
       const int n_kb = (kb1 - kb0) * s.k_passes;
-      if (!WIDE && (j & 1) != wg) {   // the other WG's tile
+      if (!WIDE && (int)(j & 1u) != wg) {   // the other WG's tile
         it += n_kb;
+        tile = next_item(j + 1);
         continue;
       }
       const int col_base = n_blk * BN;
@@ -317,8 +372,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
         prev_stage = stage;
       }
       // every MMA of this tile is issued: the other WG's next tile may take the tensor cores
-      // (only if it has one, so that every arrive meets a sync)
-      if (!WIDE && tile + tile_step < total_tiles) named_bar_arrive(other_turn_bar, 256);
+      // (only if it has one, so that every arrive meets a sync). The producer has issued this
+      // tile's last loads, so it is claiming or has claimed the next item.
+      const int next_tile = next_item(j + 1);
+      if (!WIDE && next_tile >= 0) named_bar_arrive(other_turn_bar, 256);
       wgmma_wait<0>();
 #pragma unroll
       for (int half = 0; half < NHALF; ++half) wgmma_fence_acc(acc[half]);
@@ -628,6 +685,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
           }
         }
       }
+      tile = next_tile;
     }
     // the slabs must not go away under stores still reading them; their global writes are
     // complete when the grid is (a dependent kernel's griddepcontrol.wait covers them)
@@ -742,20 +800,67 @@ struct GemmMaps {
   CUtensorMap a, b, out, aux, res, a_lo, b_lo;
 };
 
+// Work-item counters of the dynamic scheduler: two uint32 per (device, stream), claims and
+// retired CTAs. A launch finds them at zero and leaves them at zero (its last CTA resets them), so
+// launches need no memset and no host sync; launches on one stream are ordered by the stream and
+// pdl_wait(), and streams never share a counter, so concurrent grids do not interfere. A pair is
+// zeroed once, on its stream, when that stream first launches a GEMM.
+struct SchedSlot {
+  int device;
+  cudaStream_t stream;
+  uint32_t* counter;
+};
+constexpr int SCHED_CHUNK = 256;   // counter pairs per device allocation
+
+static int sched_counter(cudaStream_t st, uint32_t** out) {
+  static std::mutex mu;
+  static std::vector<SchedSlot> slots;
+  static std::vector<SchedSlot> chunks;   // (device, -, base of a SCHED_CHUNK-pair allocation)
+  int dev = 0;
+  HERO_CUDA_CHECK(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(mu);
+  for (const SchedSlot& sl : slots)
+    if (sl.device == dev && sl.stream == st) {
+      *out = sl.counter;
+      return HERO_OK;
+    }
+  int used = 0;
+  for (const SchedSlot& sl : slots) used += (sl.device == dev);
+  if (used % SCHED_CHUNK == 0) {
+    void* p = nullptr;
+    HERO_CUDA_CHECK(cudaMalloc(&p, SCHED_CHUNK * 2 * sizeof(uint32_t)));
+    chunks.push_back(SchedSlot{dev, nullptr, static_cast<uint32_t*>(p)});
+  }
+  uint32_t* base = nullptr;
+  for (const SchedSlot& c : chunks)
+    if (c.device == dev) base = c.counter;   // the newest chunk of this device
+  uint32_t* counter = base + 2 * (used % SCHED_CHUNK);
+  HERO_CUDA_CHECK(cudaMemsetAsync(counter, 0, 2 * sizeof(uint32_t), st));
+  slots.push_back(SchedSlot{dev, st, counter});
+  *out = counter;
+  return HERO_OK;
+}
+
 template <int A_MN, int B_MN, int ACT, int OUT, int RES, int BN = BLOCK_N>
 static int launch(const GemmMaps& tm, const GemmShape& s, const GemmEpilogue& e,
                   cudaStream_t stream) {
   using Cfg = GemmCfg<ACT, OUT, RES, BN>;
-  auto kern = gemm_wgmma_kernel<A_MN, B_MN, ACT, OUT, RES, BN>;
-  static bool attr_set = false;
-  if (!attr_set) {
+  // the static schedule is a kernel of its own, so grids that have the SMs to themselves run
+  // none of the ring's code
+  auto kern = s.dynamic ? gemm_wgmma_kernel<A_MN, B_MN, ACT, OUT, RES, BN, true>
+                        : gemm_wgmma_kernel<A_MN, B_MN, ACT, OUT, RES, BN, false>;
+  static bool attr_set[2] = {false, false};
+  if (!attr_set[s.dynamic]) {
     HERO_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::SMEM_BYTES));
-    attr_set = true;
+    attr_set[s.dynamic] = true;
   }
   const int total = s.num_m_blocks * s.num_n_blocks * s.k_splits;
   const int sms = sm_count();
   if (sms <= 0) return set_error(HERO_ERR_NO_DEVICE, "no CUDA device");
+  uint32_t* sched = nullptr;
+  if (s.dynamic)
+    if (int rc = sched_counter(stream, &sched)) return rc;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(total < sms ? total : sms);
   cfg.blockDim = dim3(NUM_THREADS);
@@ -766,7 +871,8 @@ static int launch(const GemmMaps& tm, const GemmShape& s, const GemmEpilogue& e,
   attr[0].val.programmaticStreamSerializationAllowed = serial_profiling() ? 0 : 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  HERO_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, tm.a, tm.b, tm.out, tm.aux, tm.res, tm.a_lo, tm.b_lo, s, e));
+  HERO_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, tm.a, tm.b, tm.out, tm.aux, tm.res, tm.a_lo, tm.b_lo, s, e,
+                                     sched));
   return HERO_OK;
 }
 
@@ -859,7 +965,19 @@ static GemmProfile g_prof;
 
 bool gemm_profile_active() { return g_prof.on; }
 
+static thread_local bool g_shared_sms = false;
+bool gemm_set_shared_sms(bool on) {
+  const bool prev = g_shared_sms;
+  g_shared_sms = on;
+  return prev;
+}
+
 }  // namespace hero
+
+extern "C" int hero_gemm_set_shared_sms(int32_t on) {
+  hero::gemm_set_shared_sms(on != 0);
+  return HERO_OK;
+}
 
 extern "C" int hero_gemm_profile_begin(void) {
   using namespace hero;
@@ -1017,6 +1135,7 @@ static int hero_gemm_bf16_impl(const hero_gemm_args* g, void* stream, int* bn_us
   s.k_splits = k_splits;
   HERO_REQUIRE((g->a_lo == nullptr) == (g->b_lo == nullptr), "a_lo and b_lo go together");
   s.k_passes = g->a_lo ? 3 : 1;
+  s.dynamic = g_shared_sms ? 1 : 0;
 
   GemmEpilogue e;
   e.bias = g->bias;

@@ -48,6 +48,7 @@ struct Gemm {
     g.drop_threshold = thr; g.drop_key = key; g.drop_scale = scale; return *this;
   }
   Gemm& f32_accumulate() { g.out_f32_accumulate = 1; return *this; }
+  Gemm& k_splits(int n) { g.k_splits = n; return *this; }
   // column sums of the stored output accumulate into p (bias gradient of the producing Linear)
   Gemm& colsum(float* p) { g.out_colsum = p; return *this; }
   int run(void* stream) { return hero_gemm_bf16(&g, stream); }
@@ -91,6 +92,22 @@ static int side_stream(SideStream** out) {
   }
   *out = &c;
   return HERO_OK;
+}
+
+// Split-K counts of the four weight gradients that run on the side stream (dW2, dW1, dWo, dWqkv).
+// The per-launch chooser minimises one GEMM's own latency; beside the dgrad chain what counts is
+// the SM-time the side stream takes, and every split-K item pays an fp32-atomic epilogue, so these
+// were picked by measured step time (DESIGN §4). 0 leaves a GEMM to the per-launch chooser.
+// HERO_WGRAD_SPLITS=a,b,c,d (development) overrides them for a sweep.
+static const int* wgrad_splits() {
+  static int sp[4] = {1, 1, 1, 1};
+  static const bool read = [] {
+    if (const char* v = getenv("HERO_WGRAD_SPLITS"))
+      sscanf(v, "%d,%d,%d,%d", &sp[0], &sp[1], &sp[2], &sp[3]);
+    return true;
+  }();
+  (void)read;
+  return sp;
 }
 
 #define HERO_TRY(expr)        \
@@ -191,8 +208,18 @@ extern "C" int hero_bert_stack_fwd(const hero_stack_args* s, void* stream) {
   return HERO_OK;
 }
 
+static int stack_bwd(const hero_stack_args* s, void* stream);
+
 extern "C" int hero_bert_stack_bwd(const hero_stack_args* s, void* stream) {
   HERO_TRY(check_stack(s, true));
+  const bool shared = !gemm_profile_active() && !serial_profiling();   // two streams
+  const bool prev = gemm_set_shared_sms(shared);
+  const int rc = stack_bwd(s, stream);
+  gemm_set_shared_sms(prev);
+  return rc;
+}
+
+static int stack_bwd(const hero_stack_args* s, void* stream) {
   const int M = s->n_tok, H = s->hidden, I = s->inter;
   const float scale = 0.125f;
   // carve the scratch buffer (bf16 elements)
@@ -231,6 +258,7 @@ extern "C" int hero_bert_stack_bwd(const hero_stack_args* s, void* stream) {
     return HERO_OK;
   };
   bool done_recorded[2] = {false, false};
+  const int* wsp = wgrad_splits();
 
   const void* dy = s->dout;
   for (int l = s->n_layers - 1; l >= 0; --l) {
@@ -263,12 +291,12 @@ extern "C" int hero_bert_stack_bwd(const hero_stack_args* s, void* stream) {
     HERO_STEP(ABL_LN_BWD, hero_ln_bwd(&ln, stream));
     HERO_TRY(publish());
     // FFN down
-    HERO_STEP(ABL_WGRAD, Gemm(g2, H, 1, A.f, I, 1, H, I, M, G.dw2, I).f32_accumulate().run(wstream));
+    HERO_STEP(ABL_WGRAD, Gemm(g2, H, 1, A.f, I, 1, H, I, M, G.dw2, I).f32_accumulate().k_splits(wsp[0]).run(wstream));
     // (its epilogue also accumulates the column sums of dpre = the FFN-up bias gradient)
     HERO_STEP(ABL_DGRAD, Gemm(g2, H, 0, W.w2, I, 1, M, I, H, dpre, I).act(ACT_GELU_GRAD).aux_in(A.pre, I).colsum(G.db1).run(stream));
     HERO_TRY(publish());
     // FFN up
-    HERO_STEP(ABL_WGRAD, Gemm(dpre, I, 1, A.a, H, 1, I, H, M, G.dw1, H).f32_accumulate().run(wstream));
+    HERO_STEP(ABL_WGRAD, Gemm(dpre, I, 1, A.a, H, 1, I, H, M, G.dw1, H).f32_accumulate().k_splits(wsp[1]).run(wstream));
     HERO_STEP(ABL_DGRAD, Gemm(dpre, I, 0, W.w1, H, 1, M, H, I, da, H).resid(ds2, H).run(stream));
     // LN1 backward
     ln_base(&ln, A.s1, W.ln1_g, nullptr, s->eps, M, H, A.mean1, A.rstd1);
@@ -285,7 +313,7 @@ extern "C" int hero_bert_stack_bwd(const hero_stack_args* s, void* stream) {
     HERO_STEP(ABL_LN_BWD, hero_ln_bwd(&ln, stream));
     HERO_TRY(publish());
     // attention output projection
-    HERO_STEP(ABL_WGRAD, Gemm(g1, H, 1, A.cx, H, 1, H, H, M, G.dwo, H).f32_accumulate().run(wstream));
+    HERO_STEP(ABL_WGRAD, Gemm(g1, H, 1, A.cx, H, 1, H, H, M, G.dwo, H).f32_accumulate().k_splits(wsp[2]).run(wstream));
     HERO_STEP(ABL_DGRAD, Gemm(g1, H, 0, W.wo, H, 1, M, H, H, dcx, H).run(stream));
     // attention core
     HERO_STEP(ABL_ATTN_BWD, hero_attn_bwd(A.qkv, s->tile_tok0, s->tile_ntok, s->seq_lo, s->seq_hi, A.cx, dcx, A.lse,
@@ -294,7 +322,7 @@ extern "C" int hero_bert_stack_bwd(const hero_stack_args* s, void* stream) {
                            site_key(s->drop_key, s->first_layer + l, 0), s->attn_drop_scale, stream));
     HERO_TRY(publish());
     // QKV projection
-    HERO_STEP(ABL_WGRAD, Gemm(dqkv, 3 * H, 1, h_in, H, 1, 3 * H, H, M, G.dwqkv, H).f32_accumulate().run(wstream));
+    HERO_STEP(ABL_WGRAD, Gemm(dqkv, 3 * H, 1, h_in, H, 1, 3 * H, H, M, G.dwqkv, H).f32_accumulate().k_splits(wsp[3]).run(wstream));
     if (two_streams) {
       HERO_CUDA_CHECK(cudaEventRecord(side->done[par], side->stream));
       done_recorded[par] = true;

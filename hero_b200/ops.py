@@ -44,6 +44,12 @@ def set_sm_limit(n):
     _lib.check(_lib.lib().hero_set_sm_limit(int(n)))
 
 
+def set_gemm_shared_sms(on):
+    """Dynamic work items for this thread's later GEMM launches (`hero_gemm_set_shared_sms`):
+    for GEMMs that share the SMs with another stream's work."""
+    _lib.check(_lib.lib().hero_gemm_set_shared_sms(int(bool(on))))
+
+
 def start_gemm_profile():
     """Bracket every GEMM launch (direct or from the layer runtime) with CUDA events on the
     launching stream (bench.py roofline); implemented in the library."""

@@ -145,6 +145,11 @@ typedef struct hero_gemm_args {
 
 int hero_gemm_bf16(const hero_gemm_args* args, void* stream);
 
+/* on != 0: this host thread's later GEMM launches claim their work items from a per-stream device
+   counter instead of a static stride (for grids that share the SMs with another stream's work;
+   hero_bert_stack_bwd sets it for its own launches). */
+int hero_gemm_set_shared_sms(int32_t on);
+
 /* Measurement aid for the roofline line of bench.py: between begin and end every GEMM launch (direct
  * or issued by the layer runtime) is bracketed by CUDA events on its stream; end synchronises and
  * returns the summed kernel time [ms], the summed 2*M*N*K [FLOP] and the number of launches. */
