@@ -173,6 +173,11 @@ def _declare(lib):
     sig("hero_qa_pool_bwd", vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp,
         vp)
     sig("hero_dec_attn_fwd", vp, i64, vp, i64, vp, i64, vp, vp, i32, i32, i32, f32, vp, i64, vp)
+    sig("hero_dec_attn_gather_fwd", vp, i64, vp, i64, vp, i64, vp, i64, vp, i32, i32, i32, i32, f32,
+        vp, i64, vp)
+    sig("hero_beam_logprob_topk", vp, i64, i32, i32, i32, vp, vp, vp, vp)
+    sig("hero_beam_select", vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp,
+        vp, vp)
 
 
 def lib():

@@ -13,6 +13,11 @@
 // tensor-core tile would be almost all padding, so the dot products run on CUDA cores in fp32:
 // one thread per key for Q.K (16-byte loads of the 64-element key row), then each warp walks a
 // quarter of the keys for P.V with every lane owning two output columns (128-byte coalesced rows).
+//
+// The gather form (hero_dec_attn_gather_fwd) is the same kernel body with key j of query row i read
+// from row kv_idx[i * ld_idx + j] instead of kv_off[i] + j: beam search addresses each beam's
+// history through its ancestry table and never copies a KV cache. Only the row lookup differs, so
+// the range form's arithmetic, and its results, are those of the kernel before the template.
 #include <cuda_bf16.h>
 #include <math.h>
 
@@ -42,11 +47,15 @@ __device__ __forceinline__ float da_block_reduce(float v, float* red, bool is_ma
   return r;
 }
 
+// GATHER: key j of row i is row kv_idx[i * ld_idx + j] (checked against [0, n_kv)); otherwise
+// row kv_off[i] + j (kv_idx, ld_idx and n_kv unused).
+template <bool GATHER>
 __global__ void __launch_bounds__(DA_THREADS)
     dec_attn_fwd_kernel(const __nv_bfloat16* __restrict__ q, int64_t ldq,
                         const __nv_bfloat16* __restrict__ k, int64_t ldk,
                         const __nv_bfloat16* __restrict__ v, int64_t ldv,
                         const int32_t* __restrict__ kv_off, const int32_t* __restrict__ kv_len,
+                        const int32_t* __restrict__ kv_idx, int64_t ld_idx, int32_t n_kv,
                         float scale, __nv_bfloat16* __restrict__ out, int64_t ldo) {
   __shared__ float qs[DA_HEAD_DIM];
   __shared__ float p[DA_MAX_KV];
@@ -56,7 +65,8 @@ __global__ void __launch_bounds__(DA_THREADS)
   const int col0 = head * DA_HEAD_DIM;
   pdl_wait();
   pdl_launch_dependents();
-  const int off = __ldg(kv_off + row), len = __ldg(kv_len + row);
+  const int off = GATHER ? 0 : __ldg(kv_off + row), len = __ldg(kv_len + row);
+  const int32_t* idx = GATHER ? kv_idx + (int64_t)row * ld_idx : nullptr;
   __nv_bfloat16* o = out + (int64_t)row * ldo + col0;
   if (len < 1 || len > DA_MAX_KV) {   // outside the contract: NaN, never a stray read
     if (tid < DA_HEAD_DIM) o[tid] = __float2bfloat16(__int_as_float(0x7fc00000));
@@ -67,8 +77,17 @@ __global__ void __launch_bounds__(DA_THREADS)
 
   // scores s_j = (q / sqrt(d)) . k_j, one key per thread
   float mx = -INFINITY;
+  bool bad = false;
   for (int j = tid; j < len; j += DA_THREADS) {
-    const uint4* kr = reinterpret_cast<const uint4*>(k + (int64_t)(off + j) * ldk + col0);
+    int64_t kj = off + j;
+    if constexpr (GATHER) {
+      kj = __ldg(idx + j);
+      if (kj < 0 || kj >= n_kv) {
+        bad = true;
+        continue;
+      }
+    }
+    const uint4* kr = reinterpret_cast<const uint4*>(k + kj * ldk + col0);
     float s = 0.f;
 #pragma unroll
     for (int c = 0; c < DA_HEAD_DIM / 8; ++c) {
@@ -84,6 +103,12 @@ __global__ void __launch_bounds__(DA_THREADS)
     p[j] = s;
     mx = fmaxf(mx, s);
   }
+  if constexpr (GATHER) {
+    if (__syncthreads_or(bad)) {         // a key row outside [0, n_kv): NaN, never a stray read
+      if (tid < DA_HEAD_DIM) o[tid] = __float2bfloat16(__int_as_float(0x7fc00000));
+      return;
+    }
+  }
   mx = da_block_reduce(mx, red, true);
   float sum = 0.f;
   for (int j = tid; j < len; j += DA_THREADS) {
@@ -98,8 +123,9 @@ __global__ void __launch_bounds__(DA_THREADS)
   float a0 = 0.f, a1 = 0.f;
   for (int j = warp; j < len; j += DA_WARPS) {
     const float pj = p[j];
+    const int64_t vj = GATHER ? (int64_t)__ldg(idx + j) : (int64_t)(off + j);
     const float2 f = __bfloat1622float2(
-        reinterpret_cast<const __nv_bfloat162*>(v + (int64_t)(off + j) * ldv + col0)[lane]);
+        reinterpret_cast<const __nv_bfloat162*>(v + vj * ldv + col0)[lane]);
     a0 = fmaf(pj, f.x, a0);
     a1 = fmaf(pj, f.y, a1);
   }
@@ -118,30 +144,56 @@ __global__ void __launch_bounds__(DA_THREADS)
 
 using namespace hero;
 
+namespace {
+
+int dec_attn_launch(bool gather, const void* q, int64_t ldq, const void* k, int64_t ldk,
+                    const void* v, int64_t ldv, const int32_t* kv_off, const int32_t* kv_len,
+                    const int32_t* kv_idx, int64_t ld_idx, int32_t n_kv, int32_t rows,
+                    int32_t heads, int32_t head_dim, float scale, void* out, int64_t ldo,
+                    void* stream, const char* name) {
+  HERO_REQUIRE(q && k && v && kv_len && out && (gather ? kv_idx != nullptr : kv_off != nullptr),
+               "%s: null pointer", name);
+  HERO_REQUIRE(head_dim == DA_HEAD_DIM, "%s: head_dim = %d (only %d)", name, head_dim,
+               DA_HEAD_DIM);
+  HERO_REQUIRE(rows >= 0 && heads >= 1 && heads <= 65535, "%s: rows %d, heads %d", name, rows,
+               heads);
+  const int64_t width = (int64_t)heads * head_dim;
+  HERO_REQUIRE(ldq >= width && ldk >= width && ldv >= width && ldo >= width,
+               "%s: a leading dimension is below heads * head_dim = %lld", name,
+               (long long)width);
+  HERO_REQUIRE(ldk % 8 == 0 && (reinterpret_cast<uintptr_t>(k) & 15) == 0,
+               "%s: K needs 16-byte aligned rows (ldk %lld)", name, (long long)ldk);
+  HERO_REQUIRE(ldv % 2 == 0 && (reinterpret_cast<uintptr_t>(v) & 3) == 0,
+               "%s: V needs 4-byte aligned rows (ldv %lld)", name, (long long)ldv);
+  HERO_REQUIRE(!gather || (ld_idx >= 0 && n_kv >= 1), "%s: ld_idx %lld, n_kv %d", name,
+               (long long)ld_idx, n_kv);
+  if (rows == 0) return HERO_OK;
+  HERO_CUDA_CHECK(launch_pdl(gather ? dec_attn_fwd_kernel<true> : dec_attn_fwd_kernel<false>,
+                             dim3(rows, heads), dim3(DA_THREADS), 0,
+                             reinterpret_cast<cudaStream_t>(stream),
+                             static_cast<const __nv_bfloat16*>(q), ldq,
+                             static_cast<const __nv_bfloat16*>(k), ldk,
+                             static_cast<const __nv_bfloat16*>(v), ldv, kv_off, kv_len, kv_idx,
+                             ld_idx, n_kv, scale, static_cast<__nv_bfloat16*>(out), ldo));
+  return HERO_OK;
+}
+
+}  // namespace
+
 extern "C" int hero_dec_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk,
                                  const void* v, int64_t ldv, const int32_t* kv_off,
                                  const int32_t* kv_len, int32_t rows, int32_t heads,
                                  int32_t head_dim, float scale, void* out, int64_t ldo,
                                  void* stream) {
-  HERO_REQUIRE(q && k && v && kv_off && kv_len && out, "dec_attn_fwd: null pointer");
-  HERO_REQUIRE(head_dim == DA_HEAD_DIM, "dec_attn_fwd: head_dim = %d (only %d)", head_dim,
-               DA_HEAD_DIM);
-  HERO_REQUIRE(rows >= 0 && heads >= 1 && heads <= 65535, "dec_attn_fwd: rows %d, heads %d",
-               rows, heads);
-  const int64_t width = (int64_t)heads * head_dim;
-  HERO_REQUIRE(ldq >= width && ldk >= width && ldv >= width && ldo >= width,
-               "dec_attn_fwd: a leading dimension is below heads * head_dim = %lld",
-               (long long)width);
-  HERO_REQUIRE(ldk % 8 == 0 && (reinterpret_cast<uintptr_t>(k) & 15) == 0,
-               "dec_attn_fwd: K needs 16-byte aligned rows (ldk %lld)", (long long)ldk);
-  HERO_REQUIRE(ldv % 2 == 0 && (reinterpret_cast<uintptr_t>(v) & 3) == 0,
-               "dec_attn_fwd: V needs 4-byte aligned rows (ldv %lld)", (long long)ldv);
-  if (rows == 0) return HERO_OK;
-  HERO_CUDA_CHECK(launch_pdl(dec_attn_fwd_kernel, dim3(rows, heads), dim3(DA_THREADS), 0,
-                             reinterpret_cast<cudaStream_t>(stream),
-                             static_cast<const __nv_bfloat16*>(q), ldq,
-                             static_cast<const __nv_bfloat16*>(k), ldk,
-                             static_cast<const __nv_bfloat16*>(v), ldv, kv_off, kv_len, scale,
-                             static_cast<__nv_bfloat16*>(out), ldo));
-  return HERO_OK;
+  return dec_attn_launch(false, q, ldq, k, ldk, v, ldv, kv_off, kv_len, nullptr, 0, 0, rows, heads,
+                         head_dim, scale, out, ldo, stream, "dec_attn_fwd");
+}
+
+extern "C" int hero_dec_attn_gather_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk,
+                                        const void* v, int64_t ldv, const int32_t* kv_idx,
+                                        int64_t ld_idx, const int32_t* kv_len, int32_t n_kv,
+                                        int32_t rows, int32_t heads, int32_t head_dim, float scale,
+                                        void* out, int64_t ldo, void* stream) {
+  return dec_attn_launch(true, q, ldq, k, ldk, v, ldv, nullptr, kv_len, kv_idx, ld_idx, n_kv,
+                         rows, heads, head_dim, scale, out, ldo, stream, "dec_attn_gather_fwd");
 }

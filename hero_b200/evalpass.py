@@ -1200,19 +1200,26 @@ def validate_pretrain(model, val_dataloaders, opts):
     return out
 
 
-def decode_tvc(model, loader, *, max_step, bos, eos, tokenizer):
+def decode_tvc(model, loader, *, max_step, bos, eos, tokenizer, beam_size=1, length_penalty=0.0):
     """inf_tvc.py:83-98 / train_tvc.py:259-283 (decode / validate): greedy captions of every
-    segment of every batch (tvc.TvcGenerator, one device->host copy per batch) as
+    segment of every batch (tvc.TvcGenerator, one device->host copy per batch), or with
+    `beam_size` > 1 the beam-search captions of TvcGenerator.beam_search (score / len **
+    `length_penalty`), as
     `{'vid_name', 'clip_id', 'ts', 'descs': [{'desc': caption}]}` records, in batch order. The
     tokenizer is any object with `convert_ids_to_tokens` / `convert_tokens_to_string`.
     Data-parallel, every rank returns the records of all ranks, gathered with all_gather_list in
     rank order (train_tvc.py:274). The COCO caption metrics are left to the caller."""
     from .tvc import TvcGenerator
+    if not float(length_penalty) >= 0.0:
+        raise ValueError(f"length_penalty = {length_penalty}: must be >= 0")
     generator = TvcGenerator(model, max_step, bos, eos, fp16=False)
     model.eval()
     results = []
     for batch in loader:
-        outputs = generator.greedy_decode(batch)
+        if beam_size == 1:
+            outputs = generator.greedy_decode(batch)
+        else:
+            outputs = generator.beam_search(batch, beam_size, length_penalty)
         for vid, cid, ts, out_ids in zip(batch["vid_names"], batch["clip_ids"], batch["all_ts"],
                                          outputs):
             output = tokenizer.convert_tokens_to_string(tokenizer.convert_ids_to_tokens(out_ids))

@@ -890,3 +890,86 @@ def dec_attn_fwd(q, k, v, kv_off, kv_len, out, *, heads, max_kv_len, min_kv_len=
                                             head_dim, 1.0 / (head_dim ** 0.5), _ptr(out),
                                             out.stride(0), _stream()))
     return out
+
+
+def dec_attn_gather_fwd(q, k, v, kv_idx, kv_len, out, *, heads, max_kv_len, min_kv_len=1,
+                        head_dim=DEC_HEAD_DIM):
+    """dec_attn_fwd with gathered keys (`hero_dec_attn_gather_fwd`): key j of row i is row
+    kv_idx[i, j] of k / v for j < kv_len[i]. kv_idx: int32 [rows, >= max_kv_len] with unit column
+    stride (its row stride is the index leading dimension); every index must lie in [0, rows of k
+    and v), else the row comes out NaN."""
+    rows = out.shape[0]
+    if rows < 0 or heads < 1 or head_dim != DEC_HEAD_DIM or not 1 <= min_kv_len <= max_kv_len \
+            or max_kv_len > DEC_MAX_KV:
+        raise ValueError(f"dec_attn_gather_fwd: (rows, heads, head_dim, kv_len range) = ({rows}, "
+                         f"{heads}, {head_dim}, [{min_kv_len}, {max_kv_len}]); the kernel takes "
+                         f"head_dim {DEC_HEAD_DIM} and 1 to {DEC_MAX_KV} keys")
+    if kv_idx.dim() != 2 or kv_idx.shape[0] < rows or kv_idx.shape[1] < max_kv_len:
+        raise ValueError(f"dec_attn_gather_fwd: kv_idx {tuple(kv_idx.shape)} does not cover {rows} "
+                         f"rows of {max_kv_len} keys")
+    _require_cuda(q, k, v, kv_idx, kv_len, out)
+    for t in (q, k, v, out):
+        assert t.dtype == BF16 and t.dim() == 2 and t.stride(1) == 1
+        assert t.shape[1] >= heads * head_dim
+    assert q.shape[0] >= rows
+    assert kv_idx.dtype == torch.int32 and kv_idx.stride(1) == 1
+    assert kv_len.dtype == torch.int32 and kv_len.is_contiguous() and kv_len.numel() >= rows
+    _count()
+    _lib.check(_lib.lib().hero_dec_attn_gather_fwd(
+        _ptr(q), q.stride(0), _ptr(k), k.stride(0), _ptr(v), v.stride(0), _ptr(kv_idx),
+        kv_idx.stride(0), _ptr(kv_len), min(k.shape[0], v.shape[0]), rows, heads, head_dim,
+        1.0 / (head_dim ** 0.5), _ptr(out), out.stride(0), _stream()))
+    return out
+
+
+# ---------------------------------------------------------------------------------------------
+# TVC beam search (hero_b200/csrc/beam.cu)
+BEAM_MAX = 16
+
+
+def beam_logprob_topk(x, n, beam, lse, logp, cols):
+    """Per row of x (fp32, row stride x.stride(0)) over its first n columns, one read of the row:
+    lse [rows] = logsumexp, logp / cols [rows, beam] = top-`beam` (x - lse, column), descending,
+    ties to the lower column (`hero_beam_logprob_topk`)."""
+    if not 1 <= beam <= min(BEAM_MAX, n) or not 1 <= n <= x.shape[1]:
+        raise ValueError(f"beam_logprob_topk: beam {beam}, n {n} of {x.shape[1]} columns; the "
+                         f"kernel takes 1 <= beam <= {BEAM_MAX} and beam <= n")
+    _require_cuda(x, lse, logp, cols)
+    rows = x.shape[0]
+    assert x.dtype == torch.float32 and x.stride(1) == 1
+    assert lse.dtype == torch.float32 and lse.is_contiguous() and lse.numel() >= rows
+    for t, dt in ((logp, torch.float32), (cols, torch.int32)):
+        assert t.dtype == dt and t.is_contiguous() and t.numel() >= rows * beam
+    _count()
+    _lib.check(_lib.lib().hero_beam_logprob_topk(_ptr(x), x.stride(0), rows, n, beam, _ptr(lse),
+                                                 _ptr(logp), _ptr(cols), _stream()))
+
+
+def beam_select(logp, cols, state_in, anc_in, state_out, anc_out, next_ids, *, beam, step,
+                max_step, eos):
+    """One beam-search step over logp / cols [R, beam] of beam_logprob_topk (`hero_beam_select`):
+    R = n_captions * beam rows, caption-major. `state_in` / `state_out` are (score fp32 [R],
+    finished int32 [R], length int32 [R], token history int32 [R, max_step]); anc_in / anc_out the
+    int32 [R, max_step] KV-cache row tables; next_ids int32 [R] receives the emitted tokens. Reads
+    the *_in buffers and writes the *_out ones, which must be distinct."""
+    R = logp.shape[0]
+    if not 1 <= beam <= BEAM_MAX or R % beam or not 0 <= step < max_step:
+        raise ValueError(f"beam_select: beam {beam} over {R} rows, step {step} of {max_step}; "
+                         f"the kernel takes 1 <= beam <= {BEAM_MAX} and whole captions")
+    score_i, fin_i, len_i, hist_i = state_in
+    score_o, fin_o, len_o, hist_o = state_out
+    _require_cuda(logp, cols, score_i, anc_in, score_o, anc_out, next_ids)
+    assert logp.dtype == torch.float32 and cols.dtype == torch.int32
+    for t in (logp, cols):
+        assert t.is_contiguous() and t.numel() == R * beam
+    for t in (score_i, score_o):
+        assert t.dtype == torch.float32 and t.is_contiguous() and t.numel() == R
+    for t in (fin_i, len_i, fin_o, len_o, next_ids):
+        assert t.dtype == torch.int32 and t.is_contiguous() and t.numel() == R
+    for t in (hist_i, hist_o, anc_in, anc_out):
+        assert t.dtype == torch.int32 and t.is_contiguous() and t.numel() == R * max_step
+    _count()
+    _lib.check(_lib.lib().hero_beam_select(
+        _ptr(logp), _ptr(cols), _ptr(score_i), _ptr(fin_i), _ptr(len_i), _ptr(hist_i), _ptr(anc_in),
+        R // beam, beam, step, max_step, eos, _ptr(score_o), _ptr(fin_o), _ptr(len_o), _ptr(hist_o),
+        _ptr(anc_out), _ptr(next_ids), _stream()))

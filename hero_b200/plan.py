@@ -674,6 +674,28 @@ class TvcPlan:
                 "step_len": np.repeat(t + 1, n).astype(np.int32),
                 "step_pos": np.repeat(t, n).astype(np.int32)}
 
+    def beam_arrays(self, max_step, beam):
+        """Index arrays of beam search over R = n_seg * beam rows (row n * beam + b is beam b of
+        caption n) with a KV cache laid out [max_step, R, *]: each caption's cross-attention range
+        repeated per beam (`beam_kv_off` / `beam_kv_len` [R]), per-step position ids and
+        self-attention lengths (`beam_step_pos` / `beam_step_len` [max_step, R]: t and t + 1), the
+        initial state `beam_state0` in the layout of one beam-state buffer (token history [R,
+        max_step] zeros, then the scores' fp32 bits (0 for beam 0, -inf for the others), finished
+        flags and lengths [R] each, zeros), and the initial KV-ancestry table `beam_anc0` [R,
+        max_step] whose column 0 is the row each beam writes at step 0, r."""
+        R, T = self.n_seg * beam, max_step
+        t = np.arange(T, dtype=np.int32)
+        score = np.where(np.arange(R) % beam == 0, 0.0, -np.inf).astype(np.float32)
+        anc = np.zeros((R, T), np.int32)
+        anc[:, 0] = np.arange(R, dtype=np.int32)
+        return {"beam_kv_off": np.repeat(self.kv_off, beam).astype(np.int32),
+                "beam_kv_len": np.repeat(self.kv_len, beam).astype(np.int32),
+                "beam_step_pos": np.repeat(t, R).astype(np.int32),
+                "beam_step_len": np.repeat(t + 1, R).astype(np.int32),
+                "beam_state0": np.concatenate([np.zeros(R * T, np.int32), score.view(np.int32),
+                                               np.zeros(2 * R, np.int32)]),
+                "beam_anc0": anc.reshape(-1)}
+
     def forced_arrays(self, length):
         """Index arrays of a teacher-forced pass over (n_seg, length) caption rows, row-major:
         causal self-attention ranges and each row's cross-attention range."""

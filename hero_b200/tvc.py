@@ -15,6 +15,10 @@ segment frames, its word embedding and LM head tied to the cross-modal encoder's
 runs it one position at a time against a KV cache that the QKV GEMM writes straight into, and takes
 the argmax with `rank_topk(k=1)` into the next step's id buffer: the reference instead re-runs the
 decoder and the full-vocabulary logits over the whole prefix at every step (model/tvc.py:301-330).
+Beam search runs the same pass over n_captions x beam rows: `beam_logprob_topk` gives each row's
+log-probabilities' top-B in one read of its logits, `beam_select` picks each caption's next beams
+on the device, and self-attention gathers each beam's keys through its KV-ancestry table
+(`dec_attn_gather_fwd`), so reordering beams copies no cache.
 
 Inference only. Decoder training (its attention backward and the label-smoothed loss gradient) is
 not on the CUDA path yet: `forward` raises NotImplementedError in training mode or when it would
@@ -194,10 +198,23 @@ class HeroForTvc(HeroModel):
                 "only. Call it in eval mode under torch.no_grad().")
 
     # ------------------------------------------------------------------ decoder
-    def _positions(self, w, ws, ids, pos, n_rows, layers, self_qkv, self_rng, cross_kv, cross_rng):
+    def _self_attn_range(self, off, ln, max_len):
+        """Self-attention of a pass whose keys are the ranges [off[i], off[i] + ln[i])."""
+        heads = self.decoder.num_heads
+        return lambda q, k, v, out: ops.dec_attn_fwd(q, k, v, off, ln, out, heads=heads,
+                                                     max_kv_len=max_len)
+
+    def _self_attn_gather(self, kv_idx, ln, max_len):
+        """Self-attention of a pass whose key j of row i is cache row kv_idx[i, j], j < ln[i]."""
+        heads = self.decoder.num_heads
+        return lambda q, k, v, out: ops.dec_attn_gather_fwd(q, k, v, kv_idx, ln, out, heads=heads,
+                                                            max_kv_len=max_len)
+
+    def _positions(self, w, ws, ids, pos, n_rows, layers, self_qkv, self_attn, cross_kv, cross_rng):
         """One decoder pass over n_rows positions: embedding, every layer, LM-head transform and
         the vocabulary logits (into ws.logits). `self_qkv(l)` -> (QKV output view, K view, V view)
-        of layer l; `self_rng` / `cross_rng` = (kv_off, kv_len, max_len)."""
+        of layer l; `self_attn(q, k, v, out)` launches the self-attention (_self_attn_range /
+        _self_attn_gather); `cross_rng` = (kv_off, kv_len, max_len)."""
         H = ws.x.shape[1]
         heads = self.decoder.num_heads
         _ln(w["word"], self.emb_LayerNorm, ws.x, n_rows, y_f32=ws.x32, x_rows=ids,
@@ -205,8 +222,7 @@ class HeroForTvc(HeroModel):
         for l, lw in enumerate(layers):
             qkv, k, v = self_qkv(l)
             ops.gemm(ws.x, lw["wqkv"], qkv, bias=lw["bqkv"])
-            ops.dec_attn_fwd(qkv[:, :H], k, v, self_rng[0], self_rng[1], ws.ctx, heads=heads,
-                             max_kv_len=self_rng[2])
+            self_attn(qkv[:, :H], k, v, ws.ctx)
             ops.gemm(ws.ctx, lw["wo1"], ws.s, bias=lw["bo1"], resid=ws.x32)
             _ln(ws.s, lw["ln1"], ws.a, n_rows, y_f32=ws.a32)
             ops.gemm(ws.a, lw["wq_c"], ws.qc, bias=lw["bq_c"])
@@ -254,7 +270,7 @@ class HeroForTvc(HeroModel):
         pos = pos.expand(N, Lt).reshape(-1).to(torch.int32)
         self._positions(w, ws, ids.to(device=device).reshape(-1).to(torch.int32), pos, M,
                         w["layers"], lambda l: (qkv, qkv[:, H:2 * H], qkv[:, 2 * H:]),
-                        (tdev.tf_self_off, tdev.tf_self_len, Lt),
+                        self._self_attn_range(tdev.tf_self_off, tdev.tf_self_len, Lt),
                         cross, (tdev.tf_kv_off, tdev.tf_kv_len, tplan.max_kv))
         n_valid = w["n_valid"]
         if not compute_loss:
@@ -296,7 +312,8 @@ class TvcGenerator(object):
     path runs in bf16. `greedy_decode(batch)` returns, per caption, the greedy ids cut at the first
     EOS, like the reference; it runs a fixed `max_step` positions (no early stop) with a KV cache
     and returns the token chosen at each step, where the reference re-derives every position
-    from its last full pass (equal under causal masking)."""
+    from its last full pass (equal under causal masking). `beam_search(batch, beam_size,
+    length_penalty)` decodes with a beam on the same path (not in the reference)."""
 
     def __init__(self, model, max_step, bos, eos, fp16):
         self.model = model
@@ -338,7 +355,7 @@ class TvcGenerator(object):
             step = slice(t * N, (t + 1) * N)
             model._positions(w, ws, out[t], tdev.step_pos[step], N, w["layers"],
                              lambda l: (caches[l][:, t], rows[l][:, H:2 * H], rows[l][:, 2 * H:]),
-                             (tdev.self_off, tdev.step_len[step], t + 1),
+                             model._self_attn_range(tdev.self_off, tdev.step_len[step], t + 1),
                              cross, (tdev.kv_off, tdev.kv_len, tplan.max_kv))
             ops.rank_topk(ws.logits, n_valid, 1, vals, out[t + 1].view(N, 1))
         if device.type != "cuda":
@@ -351,6 +368,96 @@ class TvcGenerator(object):
         done.synchronize()
         return host.t()
 
+    @torch.no_grad()
+    def beam_search(self, batch, beam_size, length_penalty=0.0):
+        """Per caption, the best of `beam_size` beams (see beam_ids), cut at the first EOS."""
+        ids, _ = self.beam_ids(batch, beam_size, length_penalty)
+        return [self.cut_eos(row) for row in ids.tolist()]
+
+    @torch.no_grad()
+    def beam_ids(self, batch, beam_size, length_penalty=0.0):
+        """Beam search over `max_step` steps (no early stop): (ids [n_captions, max_step] int32,
+        score [n_captions] fp32) on the host, the chosen beam's tokens and its sum of
+        log-probabilities.
+
+        Every caption starts with beam 0 at score 0 and the other beams at -inf. At each step a
+        live beam offers its top-`beam_size` tokens (descending logit, ties to the lower id) at
+        score + log-probability, a finished beam (one that has emitted EOS) offers EOS at its
+        score, and the caption keeps the `beam_size` best candidates (ties to the lower parent *
+        beam_size + rank). The chosen beam maximises score / len ** length_penalty, len = tokens up
+        to and including the first EOS (max_step without one), ties to the lower beam. With
+        beam_size 1 this is greedy decoding up to the first EOS, after which it emits EOS.
+
+        Rows n * beam_size + b run through the decoder together; the KV cache is laid out
+        [max_step, rows, 3H] per layer and each beam reads its history through a KV-ancestry
+        table, so nothing is copied when beams are reordered. Every upload of the batch happens
+        before the loop; token histories, scores and lengths come back in one device->host copy."""
+        model, T, B = self.model, int(self.max_step), int(beam_size)
+        if not 1 <= T <= MAX_DECODE_STEP:
+            raise ValueError(f"max_step = {T}: beam search takes 1 to {MAX_DECODE_STEP} steps "
+                             f"(position table of {MAX_DECODE_STEP + 1})")
+        fe = model.v_encoder.f_encoder
+        n_valid = fe.embeddings.word_embeddings.weight.shape[0] - fe.vocab_pad
+        if not 1 <= B <= min(ops.BEAM_MAX, n_valid):
+            raise ValueError(f"beam_size = {beam_size}: beam search takes 1 to "
+                             f"{min(ops.BEAM_MAX, n_valid)} beams")
+        if not float(length_penalty) >= 0.0:
+            raise ValueError(f"length_penalty = {length_penalty}: must be >= 0")
+        model._check_inference()
+        y, tplan = model.encode(batch)
+        device = y.device
+        N = tplan.n_seg
+        R = N * B
+        tdev = tplan.to(device, tplan.beam_arrays(T, B))
+        enc = model._gather_segments(y, tplan, tdev)
+        flat, w = model._weights(device)
+        cross = model._cross_kv(w, enc)
+        ws = model._workspace(R, device)
+        H = ws.x.shape[1]
+        caches = [torch.empty(T, R, 3 * H, dtype=BF16, device=device) for _ in w["layers"]]
+        rows = [c.view(T * R, 3 * H) for c in caches]
+        # beam state, ping-pong over steps: [token history R x T | score | finished | length]
+        slabs = [torch.empty(R * T + 3 * R, dtype=torch.int32, device=device) for _ in range(2)]
+        ancs = [torch.empty(R * T, dtype=torch.int32, device=device) for _ in range(2)]
+        ids = torch.full((R,), int(self.bos), dtype=torch.int32, device=device)
+        lse = torch.empty(R, dtype=torch.float32, device=device)
+        logp = torch.empty(R, B, dtype=torch.float32, device=device)
+        cols = torch.empty(R, B, dtype=torch.int32, device=device)
+        state, anc = tdev.beam_state0, tdev.beam_anc0
+        for t in range(T):
+            step = slice(t * R, (t + 1) * R)
+            model._positions(w, ws, ids, tdev.beam_step_pos[step], R, w["layers"],
+                             lambda l: (caches[l][t], rows[l][:, H:2 * H], rows[l][:, 2 * H:]),
+                             model._self_attn_gather(anc.view(R, T), tdev.beam_step_len[step],
+                                                     t + 1),
+                             cross, (tdev.beam_kv_off, tdev.beam_kv_len, tplan.max_kv))
+            ops.beam_logprob_topk(ws.logits, n_valid, B, lse, logp, cols)
+            ops.beam_select(logp, cols, _beam_state(state, R, T), anc,
+                            _beam_state(slabs[t % 2], R, T), ancs[t % 2], ids, beam=B, step=t,
+                            max_step=T, eos=int(self.eos))
+            state, anc = slabs[t % 2], ancs[t % 2]
+        if device.type != "cuda":
+            host = state.clone()
+        else:
+            # a non-blocking copy into pinned memory and an event wait: one copy, no stream sync
+            host = torch.empty(state.shape, dtype=torch.int32, pin_memory=True)
+            host.copy_(state, non_blocking=True)
+            done = torch.cuda.Event()
+            done.record()
+            done.synchronize()
+        score, _, length, hist = _beam_state(host, R, T)
+        best = self.pick_beam(score.view(N, B).numpy(), length.view(N, B).numpy(), length_penalty)
+        sel = torch.from_numpy(np.arange(N) * B + best)
+        return hist.view(R, T)[sel].clone(), score[sel].clone()
+
+    @staticmethod
+    def pick_beam(score, length, length_penalty):
+        """Per caption (row), the beam maximising score / length ** length_penalty in fp64, ties
+        to the lower beam."""
+        norm = np.asarray(score, np.float64) / np.power(np.asarray(length, np.float64),
+                                                        float(length_penalty))
+        return np.argmax(norm, axis=1)
+
     def cut_eos(self, ids):
         out_ids = []
         for i in ids:
@@ -358,3 +465,10 @@ class TvcGenerator(object):
                 break
             out_ids.append(i)
         return out_ids
+
+
+def _beam_state(buf, R, T):
+    """(score fp32 [R], finished [R], length [R], token history [R * T]) views of one beam-state
+    buffer (int32 [R * T + 3 * R], TvcPlan.beam_arrays' `beam_state0` layout)."""
+    h = R * T
+    return buf[h:h + R].view(torch.float32), buf[h + R:h + 2 * R], buf[h + 2 * R:], buf[:h]

@@ -602,6 +602,34 @@ int hero_dec_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, co
                       int64_t ldv, const int32_t* kv_off, const int32_t* kv_len, int32_t rows,
                       int32_t heads, int32_t head_dim, float scale, void* out, int64_t ldo,
                       void* stream);
+/* hero_dec_attn_fwd with gathered keys: key j of query row i is row kv_idx[i * ld_idx + j] of K / V
+ * for j < kv_len[i] (beam search reads each beam's history through its KV-ancestry table). Same
+ * kernel body and bounds; a row whose indices leave [0, n_kv) is written as NaN. */
+int hero_dec_attn_gather_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk,
+                             const void* v, int64_t ldv, const int32_t* kv_idx, int64_t ld_idx,
+                             const int32_t* kv_len, int32_t n_kv, int32_t rows, int32_t heads,
+                             int32_t head_dim, float scale, void* out, int64_t ldo, void* stream);
+
+/* ---- TVC beam search (hero_b200/csrc/beam.cu) ----
+ * Per row of x [rows, ld] over its first n columns, one read of the row: lse[row] =
+ * log(sum_j exp(x_j)), and logp / cols [rows, beam] = the top-`beam` (x_j - lse, j) in descending
+ * order, ties to the lower column. 1 <= beam <= 16, beam <= n. */
+int hero_beam_logprob_topk(const float* x, int64_t ld, int32_t rows, int32_t n, int32_t beam,
+                           float* lse, float* logp, int32_t* cols, void* stream);
+/* One beam-search step for n_cap captions of `beam` rows each (row r = caption * beam + b, R =
+ * n_cap * beam). Live row p offers (cols[p, k], score[p] + logp[p, k]) for k < beam, a finished row
+ * offers (eos, score[p]) once; per caption the `beam` best candidates (ties to the lower p * beam +
+ * k) become the new rows in that order, with score_out, fin_out (finished once eos is emitted),
+ * len_out (steps up to and including the first eos) and next_ids (the emitted token). hist [R,
+ * max_step] (tokens) and anc [R, max_step] (KV-cache rows) are copied from the parent for columns <
+ * step (hist) / <= step (anc); hist_out[r, step] is the token and anc_out[r, step + 1] = (step + 1)
+ * * R + r. Inputs and outputs are distinct buffers (ping-pong over steps). */
+int hero_beam_select(const float* logp, const int32_t* cols, const float* score_in,
+                     const int32_t* fin_in, const int32_t* len_in, const int32_t* hist_in,
+                     const int32_t* anc_in, int32_t n_cap, int32_t beam, int32_t step,
+                     int32_t max_step, int32_t eos, float* score_out, int32_t* fin_out,
+                     int32_t* len_out, int32_t* hist_out, int32_t* anc_out, int32_t* next_ids,
+                     void* stream);
 
 #ifdef __cplusplus
 }
