@@ -178,6 +178,8 @@ def _declare(lib):
     sig("hero_beam_logprob_topk", vp, i64, i32, i32, i32, vp, vp, vp, vp)
     sig("hero_beam_select", vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp,
         vp, vp)
+    sig("hero_dec_ban_tokens", vp, i64, i32, i32, vp, i64, i64, i32, i32, i32, i32, i32, vp)
+    sig("hero_sample_tokens", vp, i64, i32, i32, f32, i32, f32, u32, i32, vp, vp)
 
 
 def lib():

@@ -9,11 +9,12 @@
 //                           (clip, start, end) triples, enumerated on the fly
 //
 // Both selections are one CTA per row: an 8-bit radix select on the order-preserving uint32 image
-// of the float finds the N-th largest key, the survivors are gathered (ties at the threshold in
-// ascending item order) and bitonic-sorted in shared memory on (key, -item). The output order is
-// therefore deterministic: descending value, ties to the lower item index.
+// of the float (radix_select.cuh) finds the N-th largest key, the survivors are gathered (ties at
+// the threshold in ascending item order) and bitonic-sorted in shared memory on (key, -item). The
+// output order is therefore deterministic: descending value, ties to the lower item index.
 #include "common.h"
 #include "ptx.cuh"
+#include "radix_select.cuh"
 
 namespace hero {
 
@@ -25,14 +26,6 @@ constexpr int RANK_MAX_KW = 15;           // span convolution width
 constexpr int MOMENT_SMEM_MAX = 160 * 1024;   // st / ed / factor staged in shared memory up to this
 constexpr float kRankMaskFill = -1e4f;    // mask_logits (model/modeling_utils.py:42-43)
 
-// float -> uint32 with the same order (negative floats reversed, positive above them)
-__device__ __forceinline__ uint32_t ord_key(float x) {
-  const uint32_t b = __float_as_uint(x);
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float key_to_float(uint32_t k) {
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
 // descending order of the packed value = descending key, then ascending item
 __device__ __forceinline__ unsigned long long pack_cand(uint32_t key, uint32_t item) {
   return ((unsigned long long)key << 32) | (unsigned long long)(0xffffffffu - item);
@@ -42,10 +35,10 @@ __device__ __forceinline__ uint32_t cand_item(unsigned long long c) {
 }
 
 struct SelectSmem {
-  uint32_t hist[256];
+  RadixSmem<uint32_t> radix;
   uint32_t warp_cnt[RANK_THREADS / 32];
   unsigned long long cand[RANK_MAX_N];
-  uint32_t prefix, need, take_all, n_atomic;
+  uint32_t n_atomic;
 };
 static_assert(MOMENT_SMEM_MAX + sizeof(SelectSmem) <= 227 * 1024,
               "staged moment selection exceeds the sm_90 shared memory per block");
@@ -57,63 +50,11 @@ template <class Src>
 __device__ int block_select_sorted(const Src& src, int n_items, int n_sel, SelectSmem& sm) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   constexpr unsigned kFull = 0xffffffffu;
-  uint32_t prefix = 0, need = (uint32_t)n_sel;
-  bool take_all = false;
-  // ---- radix select: 4 passes of 8 bits, most significant first
-  for (int pass = 0; pass < 4; ++pass) {
-    const int shift = 24 - 8 * pass;
-    const uint32_t hmask = pass == 0 ? 0u : (0xffffffffu << (shift + 8));
-    for (int i = tid; i < 256; i += RANK_THREADS) sm.hist[i] = 0;
-    __syncthreads();
-    for (int base = 0; base < n_items; base += RANK_THREADS) {   // warp-uniform trip count
-      const int t = base + tid;
-      uint32_t k = 0;
-      int bin = -1;
-      if (t < n_items && src.get(t, k) && (k & hmask) == prefix) bin = (int)((k >> shift) & 255u);
-      const unsigned peers = __match_any_sync(kFull, bin);
-      if (bin >= 0 && lane == __ffs(peers) - 1) atomicAdd(&sm.hist[bin], (uint32_t)__popc(peers));
-    }
-    __syncthreads();
-    if (warp == 0) {
-      // lane l owns bins 255 - 8l .. 248 - 8l (descending)
-      uint32_t c[8], s = 0;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        c[i] = sm.hist[255 - 8 * lane - i];
-        s += c[i];
-      }
-      uint32_t inc = s;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t v = __shfl_up_sync(kFull, inc, o);
-        if (lane >= o) inc += v;
-      }
-      const uint32_t total = __shfl_sync(kFull, inc, 31);
-      if (pass == 0 && total <= need) {          // no more items than asked for: keep them all
-        if (lane == 0) sm.take_all = 1u;
-      } else {
-        const unsigned hit = __ballot_sync(kFull, inc >= need);
-        if (lane == __ffs(hit) - 1) {
-          uint32_t acc = inc - s;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            if (acc + c[i] >= need) {
-              sm.prefix = prefix | ((uint32_t)(255 - 8 * lane - i) << shift);
-              sm.need = need - acc;
-              break;
-            }
-            acc += c[i];
-          }
-        }
-        if (lane == 0) sm.take_all = 0u;
-      }
-    }
-    __syncthreads();
-    take_all = sm.take_all != 0u;
-    if (take_all) break;
-    prefix = sm.prefix;
-    need = sm.need;
-  }
+  uint32_t prefix, need;
+  bool take_all;
+  // ---- radix select of the n_sel-th largest key (radix_select.cuh)
+  block_radix_select<RANK_THREADS, false>(src, n_items, (uint32_t)n_sel, sm.radix, prefix, need,
+                                          take_all);
   // ---- gather: keys above the threshold in any order, keys equal to it in item order
   if (tid == 0) sm.n_atomic = 0;
   __syncthreads();

@@ -21,7 +21,8 @@
   pretrain.py:387-608: the fused LM-head GEMM with `hero_ce_finish_stats` for MLM and MFM-NCE (no
   logits tensor), `hero_row_l2_cos` for l2 / cosine, sums on the device, one device->host copy per
   task (DESIGN §4 "Pretraining validation").
-* `decode_tvc` — greedy TVC captions of inf_tvc.py / train_tvc.py.
+* `decode_tvc` — TVC captions of inf_tvc.py / train_tvc.py: greedy (the reference's), beam
+  search or sampling, with optional n-gram blocking and minimum length.
 * `ModelSaver` / `TrainingRestorer` — utils/save.py:112-181 with the same file layout (`vocab_padded`
   flag, `model_step_<n>.pt`, `train_state_<n>.pt`, `restore.pt` + backup), so checkpoints are
   interchangeable with the reference's; optimizer state is FusedAdamW's flat moments.
@@ -1200,23 +1201,37 @@ def validate_pretrain(model, val_dataloaders, opts):
     return out
 
 
-def decode_tvc(model, loader, *, max_step, bos, eos, tokenizer, beam_size=1, length_penalty=0.0):
+def decode_tvc(model, loader, *, max_step, bos, eos, tokenizer, beam_size=1, length_penalty=0.0,
+               min_length=0, no_repeat_ngram_size=0, do_sample=False, temperature=1.0, top_k=0,
+               top_p=1.0, seed=0):
     """inf_tvc.py:83-98 / train_tvc.py:259-283 (decode / validate): greedy captions of every
     segment of every batch (tvc.TvcGenerator, one device->host copy per batch), or with
     `beam_size` > 1 the beam-search captions of TvcGenerator.beam_search (score / len **
-    `length_penalty`), as
+    `length_penalty`), or with `do_sample` one sampled caption per segment (TvcGenerator.sample
+    with `temperature`, `top_k`, `top_p`), as
     `{'vid_name', 'clip_id', 'ts', 'descs': [{'desc': caption}]}` records, in batch order. The
     tokenizer is any object with `convert_ids_to_tokens` / `convert_tokens_to_string`.
+    `min_length` and `no_repeat_ngram_size` apply to every strategy (TvcGenerator). Batch i of
+    rank r samples under tvc.sampling_seed(seed, r, i), so no two batches share their uniforms.
     Data-parallel, every rank returns the records of all ranks, gathered with all_gather_list in
     rank order (train_tvc.py:274). The COCO caption metrics are left to the caller."""
-    from .tvc import TvcGenerator
+    from .tvc import TvcGenerator, _check_seed, sampling_seed
     if not float(length_penalty) >= 0.0:
         raise ValueError(f"length_penalty = {length_penalty}: must be >= 0")
-    generator = TvcGenerator(model, max_step, bos, eos, fp16=False)
+    if do_sample and beam_size != 1:
+        raise ValueError(f"do_sample with beam_size = {beam_size}: sampling draws one caption per "
+                         f"segment and takes beam_size 1")
+    _check_seed(seed)
+    generator = TvcGenerator(model, max_step, bos, eos, fp16=False, min_length=min_length,
+                             no_repeat_ngram_size=no_repeat_ngram_size)
     model.eval()
+    rank = distributed.rank()
     results = []
-    for batch in loader:
-        if beam_size == 1:
+    for i, batch in enumerate(loader):
+        if do_sample:
+            outputs = generator.sample(batch, temperature=temperature, top_k=top_k, top_p=top_p,
+                                       seed=sampling_seed(seed, rank, i))
+        elif beam_size == 1:
             outputs = generator.greedy_decode(batch)
         else:
             outputs = generator.beam_search(batch, beam_size, length_penalty)

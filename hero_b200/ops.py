@@ -5,6 +5,7 @@ Every wrapper enqueues on torch's current CUDA stream, which is what the referen
 PrefetchLoader has already synchronised the inputs against (data/loader.py:135-138).
 """
 import ctypes as C
+import math
 
 import torch
 
@@ -973,3 +974,55 @@ def beam_select(logp, cols, state_in, anc_in, state_out, anc_out, next_ids, *, b
         _ptr(logp), _ptr(cols), _ptr(score_i), _ptr(fin_i), _ptr(len_i), _ptr(hist_i), _ptr(anc_in),
         R // beam, beam, step, max_step, eos, _ptr(score_o), _ptr(fin_o), _ptr(len_o), _ptr(hist_o),
         _ptr(anc_out), _ptr(next_ids), _stream()))
+
+
+# ---------------------------------------------------------------------------------------------
+# TVC decoding controls (hero_b200/csrc/decode_ctl.cu)
+BAN_MAX_HIST = 1024
+SAMPLE_MAX_COLS = 52 * 1024
+
+
+def ban_tokens(x, n_valid, hist, *, step_stride, row_stride, bos, step, ngram, min_length, eos):
+    """-inf into the logits x [rows, >= n_valid] (fp32) of the tokens banned at decode step `step`
+    (`hero_dec_ban_tokens`): those that would repeat an `ngram`-gram of s = [bos, history] and, while
+    step < min_length, eos. Row r's history token j < step is hist.view(-1)[j * step_stride +
+    r * row_stride] (int32). A step at which neither rule applies launches nothing."""
+    rows = x.shape[0]
+    if ngram < 0 or min_length < 0 or not 0 <= step < BAN_MAX_HIST \
+            or not 1 <= n_valid <= x.shape[1]:
+        raise ValueError(f"ban_tokens: ngram {ngram}, min_length {min_length}, step {step}, "
+                         f"n_valid {n_valid} of {x.shape[1]} columns; the kernel takes ngram, "
+                         f"min_length >= 0 and steps below {BAN_MAX_HIST}")
+    if rows and step > 0 and hist.numel() <= (rows - 1) * row_stride + (step - 1) * step_stride:
+        raise ValueError(f"ban_tokens: a history of {hist.numel()} tokens does not hold {rows} rows "
+                         f"of {step} steps at strides ({row_stride}, {step_stride})")
+    if ngram == 0 and step >= min_length:
+        return
+    _require_cuda(x, hist)
+    assert x.dtype == torch.float32 and x.stride(1) == 1
+    assert hist.dtype == torch.int32 and hist.is_contiguous()
+    _count()
+    _lib.check(_lib.lib().hero_dec_ban_tokens(_ptr(x), x.stride(0), rows, n_valid, _ptr(hist),
+                                              step_stride, row_stride, bos, step, ngram,
+                                              min_length, eos, _stream()))
+
+
+def sample_tokens(x, n, ids, *, temperature, top_k, top_p, seed, step):
+    """ids [rows] (int32) = one column per row of x (fp32, row stride x.stride(0)) over its first
+    n columns, drawn by Gumbel-max after temperature, top-k and top-p (`hero_sample_tokens`;
+    csrc/decode_ctl.cu states the rules and the random key (seed, row, step))."""
+    if not 1 <= n <= min(SAMPLE_MAX_COLS, x.shape[1]) or not temperature > 0.0 \
+            or not math.isfinite(temperature) or top_k < 0 or not 0.0 < top_p <= 1.0 \
+            or not 0 <= seed < 2 ** 32 or step < 0:
+        raise ValueError(f"sample_tokens: n {n} of {x.shape[1]} columns, temperature "
+                         f"{temperature}, top_k {top_k}, top_p {top_p}, seed {seed}, step {step}; "
+                         f"the kernel takes n <= {SAMPLE_MAX_COLS}, temperature > 0, top_k >= 0, "
+                         f"0 < top_p <= 1 and a 32-bit seed")
+    _require_cuda(x, ids)
+    rows = x.shape[0]
+    assert x.dtype == torch.float32 and x.stride(1) == 1
+    assert ids.dtype == torch.int32 and ids.is_contiguous() and ids.numel() >= rows
+    _count()
+    _lib.check(_lib.lib().hero_sample_tokens(_ptr(x), x.stride(0), rows, n, float(temperature),
+                                             int(top_k), float(top_p), int(seed), step, _ptr(ids),
+                                             _stream()))

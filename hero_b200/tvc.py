@@ -18,7 +18,10 @@ decoder and the full-vocabulary logits over the whole prefix at every step (mode
 Beam search runs the same pass over n_captions x beam rows: `beam_logprob_topk` gives each row's
 log-probabilities' top-B in one read of its logits, `beam_select` picks each caption's next beams
 on the device, and self-attention gathers each beam's keys through its KV-ancestry table
-(`dec_attn_gather_fwd`), so reordering beams copies no cache.
+(`dec_attn_gather_fwd`), so reordering beams copies no cache. Sampling runs greedy decoding's loop
+with `sample_tokens` (temperature, top-k, top-p and a Gumbel-max draw keyed by (seed, row, step))
+in place of the argmax, and the decoding controls (no_repeat_ngram_size, min_length) write -inf
+into each step's logits with `ban_tokens` before any of the three selections.
 
 Inference only. Decoder training (its attention backward and the label-smoothed loss gradient) is
 not on the CUDA path yet: `forward` raises NotImplementedError in training mode or when it would
@@ -313,14 +316,46 @@ class TvcGenerator(object):
     EOS, like the reference; it runs a fixed `max_step` positions (no early stop) with a KV cache
     and returns the token chosen at each step, where the reference re-derives every position
     from its last full pass (equal under causal masking). `beam_search(batch, beam_size,
-    length_penalty)` decodes with a beam on the same path (not in the reference)."""
+    length_penalty)` decodes with a beam and `sample(batch, ...)` draws one caption per segment, on
+    the same path (neither is in the reference).
 
-    def __init__(self, model, max_step, bos, eos, fp16):
+    Decoding controls, applied by every method to the logits of each step before the selection
+    (`ops.ban_tokens`; 0 turns a control off, and with both off no kernel runs for them):
+    `no_repeat_ngram_size` n bans every token that would complete an n-gram already present in
+    [bos] + the row's history, and `min_length` bans EOS at the steps t < min_length. A banned
+    token gets logit -inf, so its probability is 0 and the others are renormalised (beam scores
+    included)."""
+
+    def __init__(self, model, max_step, bos, eos, fp16, *, min_length=0, no_repeat_ngram_size=0):
         self.model = model
         self.max_step = max_step
         self.bos = bos
         self.eos = eos
         self.fp16 = fp16
+        self.min_length = min_length
+        self.no_repeat_ngram_size = no_repeat_ngram_size
+
+    def _n_valid(self):
+        fe = self.model.v_encoder.f_encoder
+        return fe.embeddings.word_embeddings.weight.shape[0] - fe.vocab_pad
+
+    def _check_controls(self, n_valid):
+        """The controls' bounds: at most max_step n-gram bans and EOS fall on one row, so
+        max_step + 2 columns guarantee that a row is never fully masked."""
+        n, m = self.no_repeat_ngram_size, self.min_length
+        if int(n) != n or n < 0:
+            raise ValueError(f"no_repeat_ngram_size = {n}: must be an integer >= 0")
+        if int(m) != m or m < 0:
+            raise ValueError(f"min_length = {m}: must be an integer >= 0")
+        if (n or m) and int(self.max_step) + 2 > n_valid:
+            raise ValueError(f"max_step = {self.max_step}: with no_repeat_ngram_size or min_length "
+                             f"on, max_step + 2 must not exceed the {n_valid} vocabulary entries")
+
+    def _ban(self, logits, n_valid, hist, step_stride, row_stride, t):
+        if self.no_repeat_ngram_size or self.min_length:
+            ops.ban_tokens(logits, n_valid, hist, step_stride=step_stride, row_stride=row_stride,
+                           bos=int(self.bos), step=t, ngram=int(self.no_repeat_ngram_size),
+                           min_length=int(self.min_length), eos=int(self.eos))
 
     @torch.no_grad()
     def greedy_decode(self, batch):
@@ -331,10 +366,44 @@ class TvcGenerator(object):
     def decode_ids(self, batch):
         """Greedy ids (n_captions, max_step) as a host int32 tensor. Every upload of the batch
         happens before the loop; the ids come back in one device->host copy."""
+        return self._decode_rows(batch, "greedy decoding", None)
+
+    @torch.no_grad()
+    def sample(self, batch, *, temperature=1.0, top_k=0, top_p=1.0, seed=0):
+        """Per caption, one sampled caption (see sample_ids), cut at the first EOS."""
+        ids = self.sample_ids(batch, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed)
+        return [self.cut_eos(row) for row in ids.tolist()]
+
+    @torch.no_grad()
+    def sample_ids(self, batch, *, temperature=1.0, top_k=0, top_p=1.0, seed=0):
+        """Sampled ids (n_captions, max_step) as a host int32 tensor: greedy decoding's loop with
+        `ops.sample_tokens` in place of the argmax. Each step divides the logits by `temperature`,
+        keeps the columns at or above the `top_k`-th largest (0: all), then the smallest set of the
+        largest columns whose probability reaches `top_p` (1: all), and draws from the
+        renormalised distribution by Gumbel-max. The uniforms are a hash of (seed, caption row,
+        step, column), so the same batch and seed give the same ids (csrc/decode_ctl.cu). One
+        upload before the loop, one device->host copy after it."""
+        if not (float(temperature) > 0.0 and math.isfinite(float(temperature))):
+            raise ValueError(f"temperature = {temperature}: must be > 0")
+        if int(top_k) != top_k or top_k < 0:
+            raise ValueError(f"top_k = {top_k}: must be an integer >= 0 (0 keeps every token)")
+        if not 0.0 < float(top_p) <= 1.0:
+            raise ValueError(f"top_p = {top_p}: must lie in (0, 1] (1 keeps every token)")
+        _check_seed(seed)
+        if self._n_valid() > ops.SAMPLE_MAX_COLS:
+            raise ValueError(f"{self._n_valid()} vocabulary entries: sampling takes at most "
+                             f"{ops.SAMPLE_MAX_COLS}")
+        return self._decode_rows(batch, "sampling", dict(
+            temperature=float(temperature), top_k=int(top_k), top_p=float(top_p), seed=int(seed)))
+
+    def _decode_rows(self, batch, what, sampling):
+        """The one-row-per-caption loop of greedy decoding and sampling: `sampling` None picks the
+        argmax with rank_topk(k=1), else ops.sample_tokens with these keyword arguments."""
         model, T = self.model, int(self.max_step)
         if not 1 <= T <= MAX_DECODE_STEP:
-            raise ValueError(f"max_step = {T}: greedy decoding takes 1 to {MAX_DECODE_STEP} steps "
+            raise ValueError(f"max_step = {T}: {what} takes 1 to {MAX_DECODE_STEP} steps "
                              f"(position table of {MAX_DECODE_STEP + 1})")
+        self._check_controls(self._n_valid())
         model._check_inference()
         y, tplan = model.encode(batch)
         device = y.device
@@ -357,7 +426,12 @@ class TvcGenerator(object):
                              lambda l: (caches[l][:, t], rows[l][:, H:2 * H], rows[l][:, 2 * H:]),
                              model._self_attn_range(tdev.self_off, tdev.step_len[step], t + 1),
                              cross, (tdev.kv_off, tdev.kv_len, tplan.max_kv))
-            ops.rank_topk(ws.logits, n_valid, 1, vals, out[t + 1].view(N, 1))
+            # history token j of caption n is out[1 + j, n]
+            self._ban(ws.logits, n_valid, out[1:], N, 1, t)
+            if sampling is None:
+                ops.rank_topk(ws.logits, n_valid, 1, vals, out[t + 1].view(N, 1))
+            else:
+                ops.sample_tokens(ws.logits, n_valid, out[t + 1], step=t, **sampling)
         if device.type != "cuda":
             return out[1:].t().clone()
         # a non-blocking copy into pinned memory and an event wait: one copy, no stream sync
@@ -396,13 +470,13 @@ class TvcGenerator(object):
         if not 1 <= T <= MAX_DECODE_STEP:
             raise ValueError(f"max_step = {T}: beam search takes 1 to {MAX_DECODE_STEP} steps "
                              f"(position table of {MAX_DECODE_STEP + 1})")
-        fe = model.v_encoder.f_encoder
-        n_valid = fe.embeddings.word_embeddings.weight.shape[0] - fe.vocab_pad
+        n_valid = self._n_valid()
         if not 1 <= B <= min(ops.BEAM_MAX, n_valid):
             raise ValueError(f"beam_size = {beam_size}: beam search takes 1 to "
                              f"{min(ops.BEAM_MAX, n_valid)} beams")
         if not float(length_penalty) >= 0.0:
             raise ValueError(f"length_penalty = {length_penalty}: must be >= 0")
+        self._check_controls(n_valid)
         model._check_inference()
         y, tplan = model.encode(batch)
         device = y.device
@@ -431,6 +505,8 @@ class TvcGenerator(object):
                              model._self_attn_gather(anc.view(R, T), tdev.beam_step_len[step],
                                                      t + 1),
                              cross, (tdev.beam_kv_off, tdev.beam_kv_len, tplan.max_kv))
+            # each live beam's own history: token j of row r is hist[r * T + j]
+            self._ban(ws.logits, n_valid, _beam_state(state, R, T)[3], 1, T, t)
             ops.beam_logprob_topk(ws.logits, n_valid, B, lse, logp, cols)
             ops.beam_select(logp, cols, _beam_state(state, R, T), anc,
                             _beam_state(slabs[t % 2], R, T), ancs[t % 2], ids, beam=B, step=t,
@@ -465,6 +541,30 @@ class TvcGenerator(object):
                 break
             out_ids.append(i)
         return out_ids
+
+
+def sampling_seed(seed, rank, index):
+    """The 32-bit sampling seed of batch `index` of data-parallel rank `rank` under the user's
+    `seed` (an integer in [0, 2**32)): hash_u32(hash_u32(seed, rank), index) with the dropout hash
+    of csrc/ptx.cuh, so no two (rank, batch) pairs draw from the same uniforms."""
+    _check_seed(seed)
+    return _hash_u32(_hash_u32(int(seed), rank), index)
+
+
+def _check_seed(seed):
+    if int(seed) != seed or not 0 <= seed < 2 ** 32:
+        raise ValueError(f"seed = {seed}: must be an integer in [0, 2**32)")
+
+
+def _hash_u32(key, idx):
+    m = 0xFFFFFFFF
+    h = ((idx * 0x9E3779B1) & m) ^ key
+    h ^= h >> 16
+    h = (h * 0x85EBCA6B) & m
+    h ^= h >> 13
+    h = (h * 0xC2B2AE35) & m
+    h ^= h >> 16
+    return h
 
 
 def _beam_state(buf, R, T):

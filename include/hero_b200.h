@@ -631,6 +631,29 @@ int hero_beam_select(const float* logp, const int32_t* cols, const float* score_
                      int32_t* len_out, int32_t* hist_out, int32_t* anc_out, int32_t* next_ids,
                      void* stream);
 
+/* ---- TVC decoding controls (hero_b200/csrc/decode_ctl.cu) ----
+ * Token bans at decode step `step` (0 <= step < 1024), one CTA per row r < rows of the fp32 logits
+ * x [rows, ld]. The row's history is y_j = hist[j * step_stride + r * row_stride], j < step, and
+ * s = [bos, y_0, ..., y_{step-1}] (length L = step + 1). With ngram = n >= 1 and L >= n, token
+ * s[j + n - 1] is banned for every j in [0, L - n] with s[j .. j + n - 2] == s[L - n + 1 .. L - 1]
+ * (n == 1: every token of s); with step < min_length, eos is banned. A banned column c < n_valid
+ * gets x[r, c] = -inf; nothing else is written. ngram = 0 and min_length = 0 turn the rules off;
+ * a step at which neither applies launches nothing. */
+int hero_dec_ban_tokens(float* x, int64_t ld, int32_t rows, int32_t n_valid, const int32_t* hist,
+                        int64_t step_stride, int64_t row_stride, int32_t bos, int32_t step,
+                        int32_t ngram, int32_t min_length, int32_t eos, void* stream);
+/* One sampled column per row of x [rows, ld] over its first n <= 53248 columns, written to
+ * ids[row] (int32). x / temperature, then top-k (top_k = 0 off; ties at the k-th largest kept), then
+ * top-p (top_p = 1 off; the smallest threshold set whose integer mass floor(exp(x - max) * 2^32)
+ * reaches ceil(top_p * total)), then the Gumbel-max draw argmax(x_j + G_j) over the kept columns
+ * with x_j > -inf, ties to the lower j, with G_j = -log(-log(u_j)),
+ * u_j = ((hash_u32(hash_u32(hash_u32(seed, row), step), j) >> 9) + 0.5) * 2^-23 (strictly inside
+ * (0, 1)) and hash_u32 the dropout hash. temperature > 0, top_k >= 0, 0 < top_p <= 1. The
+ * same (x, seed, step) gives the same ids bit for bit. */
+int hero_sample_tokens(const float* x, int64_t ld, int32_t rows, int32_t n, float temperature,
+                       int32_t top_k, float top_p, uint32_t seed, int32_t step, int32_t* ids,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif
