@@ -442,20 +442,12 @@ def _run_batches(model, corpus, batches, video_ids, rank_kw, want_gt, post=None)
     return qids_all, results, has_gt
 
 
-def _moment_records(score, mom, video_ids, video2idx, interval, svmr):
-    recs = []
-    keep = mom[:, 0] >= 0                     # padding past the last band-valid span
-    score, mom = score[keep], mom[keep]
-    if svmr:   # find_max_triples_from_upper_triangle_product + eval_vcmr.py:346-350 (float64)
-        st = mom[:, 1].astype(np.float64) * interval
-        ed = (mom[:, 2].astype(np.float64) + 1) * interval
-    else:      # eval_vcmr.py:396-400 (float32 frame indices)
-        st = mom[:, 1].astype(np.float32) * interval
-        ed = mom[:, 2].astype(np.float32) * interval + interval
-    for i in range(len(score)):
-        recs.append([video2idx[video_ids[int(mom[i, 0])]], float(st[i]), float(ed[i]),
-                     float(score[i])])
-    return recs
+def _top_vr(out):
+    """`_run_batches`' `post` of the prediction passes: each VR list cut on the device to the
+    first 100 clips, the ones the submission lists (eval_vcmr.py:356-360, eval_vr.py:246-249)."""
+    if "VR" in out:
+        out["VR"] = tuple(t[:, :100] for t in out["VR"])
+    return out
 
 
 def _vcmr_tasks(model, tasks):
@@ -488,28 +480,14 @@ def full_vcmr_predictions(model, corpus, batches, video_ids, video2idx, *, tasks
     Data-parallel, each rank ranks its own query batches against the whole corpus and every rank
     returns the lists of all ranks' queries, in rank order (eval_vcmr.py:125-134)."""
     tasks = _vcmr_tasks(model, tasks)
-    res = {"SVMR": [], "VCMR": [], "VR": []}
+    qids, results, has_gt = [], [], False
     if tasks:
         rank_kw = dict(tasks=tasks, q2c_alpha=q2c_alpha, max_video=max_vcmr_video,
                        min_pred_l=min_pred_l, max_pred_l=max_pred_l, max_before_nms=max_before_nms)
         qids, results, has_gt = _run_batches(model, corpus, batches, video_ids, rank_kw,
-                                             "SVMR" in tasks)
-        rows = [(r, i) for r in results for i in range(len(next(iter(r.values()))[0]))]
-        assert len(rows) == len(qids)
-        for qid, (r, i) in zip(qids, rows):
-            if "SVMR" in tasks and has_gt:
-                res["SVMR"].append(dict(desc_id=int(qid), desc="", predictions=_moment_records(
-                    *(x[i] for x in r["SVMR"]), video_ids, video2idx, vfeat_interval, True)))
-            if "VR" in r:
-                sc, ix = r["VR"][0][i][:100], r["VR"][1][i][:100]
-                res["VR"].append(dict(desc_id=int(qid), desc="", predictions=[
-                    [video2idx[video_ids[int(v)]], 0, 0, float(s)] for s, v in zip(sc, ix)]))
-            if "VCMR" in r:
-                res["VCMR"].append(dict(desc_id=int(qid), desc="", predictions=_moment_records(
-                    *(x[i] for x in r["VCMR"]), video_ids, video2idx, vfeat_interval, False)))
-    eval_res = {k: v for k, v in res.items() if len(v) != 0}
-    eval_res["video2idx"] = video2idx
-    return eval_res
+                                             "SVMR" in tasks, _top_vr)
+    return _submission([int(q) for q in qids], results, has_gt, video_ids, video2idx,
+                       vfeat_interval, [(t, t) for t in RANK_TASKS])[0]
 
 
 def full_vr_predictions(model, corpus, batches, video_ids, video2idx, *, max_vr_video=100):
@@ -518,17 +496,8 @@ def full_vr_predictions(model, corpus, batches, video_ids, video2idx, *, max_vr_
     listed as [video_idx, 0, 0, score]. Arguments and result as `full_vcmr_predictions`, also
     when data-parallel: the lists of every rank's queries, in rank order (eval_vr.py:276-293)."""
     rank_kw = dict(tasks=("VR",), q2c_alpha=None, max_video=max_vr_video)
-    qids, results, _ = _run_batches(model, corpus, batches, video_ids, rank_kw, False)
-    vr = []
-    rows = [(r, i) for r in results for i in range(len(r["VR"][0]))]
-    assert len(rows) == len(qids)
-    for qid, (r, i) in zip(qids, rows):
-        sc, ix = r["VR"][0][i][:100], r["VR"][1][i][:100]
-        vr.append(dict(desc_id=qid, desc="", predictions=[
-            [video2idx[video_ids[int(v)]], 0, 0, float(s)] for s, v in zip(sc, ix)]))
-    eval_res = {k: v for k, v in dict(VR=vr).items() if len(v) != 0}
-    eval_res["video2idx"] = video2idx
-    return eval_res
+    qids, results, _ = _run_batches(model, corpus, batches, video_ids, rank_kw, False, _top_vr)
+    return _submission(qids, results, False, video_ids, video2idx, None, [("VR", "VR")])[0]
 
 
 # ------------------------------------------------------------------ temporal NMS and TVR metrics
@@ -700,7 +669,10 @@ def eval_retrieval(submission, ground_truth, iou_thds=(0.5, 0.7), use_desc_type=
 
 
 def _packed_moments(score, mom, lookup, interval, svmr):
-    """Host arrays of one task -> (vid int64, st, ed, score, valid), times as _moment_records."""
+    """Host arrays of one task -> (vid int64, st, ed, score, valid). The list ends at its first
+    padded moment (clip row -1). Times in seconds of `interval` per frame: SVMR in float64
+    (find_max_triples_from_upper_triangle_product + eval_vcmr.py:346-350), VCMR from float32
+    frame indices (eval_vcmr.py:396-400)."""
     valid = mom[..., 0] >= 0
     vid = np.where(valid, lookup[np.maximum(mom[..., 0], 0)], 0)
     if svmr:
@@ -712,12 +684,48 @@ def _packed_moments(score, mom, lookup, interval, svmr):
     return vid, st, ed, score, valid
 
 
-def _records(qids, vid, st, ed, score, valid):
+def _records(desc_ids, vid, st, ed, score, valid):
     n = valid.sum(1).tolist()
     vid, st, ed, score = vid.tolist(), st.tolist(), ed.tolist(), score.tolist()
-    return [dict(desc_id=int(q), desc="", predictions=[
+    return [dict(desc_id=d, desc="", predictions=[
         list(r) for r in zip(vid[i][:c], st[i][:c], ed[i][:c], score[i][:c])])
-        for i, (q, c) in enumerate(zip(qids, n))]
+        for i, (d, c) in enumerate(zip(desc_ids, n))]
+
+
+def _moment_records(score, mom, video_ids, video2idx, interval, svmr):
+    """The predictions of one ranked list (score (N,), moments (N, 3)), as `_submission` lists
+    them: the same `_packed_moments` / `_records` code on a one-row batch."""
+    lookup = np.array([video2idx[v] for v in video_ids], dtype=np.int64)
+    packed = _packed_moments(np.asarray(score)[None], np.asarray(mom)[None], lookup, interval, svmr)
+    return _records([None], *packed)[0]["predictions"]
+
+
+def _submission(desc_ids, results, has_gt, video_ids, video2idx, interval, keys):
+    """The submission of `_run_batches`' per-batch host results: for each (task, result key) of
+    `keys` that has results, the task's list of dict(desc_id, desc, predictions), one per entry of
+    `desc_ids`, predictions [video_idx, st, ed, score] ([video_idx, 0, 0, score] for VR); tasks in
+    SVMR, VCMR, VR order, empty ones dropped (SVMR also without ground truth), then "video2idx".
+    Also returns what `_metrics` scores: {task: (desc_ids, vid, st, ed as float32, valid)}."""
+    lookup = np.array([video2idx[v] for v in video_ids], dtype=np.int64)
+    sub, packed = {}, {}
+    for task, key in keys:
+        parts = [r[key] for r in results if key in r]
+        if not parts or not desc_ids or (task == "SVMR" and not has_gt):
+            continue
+        score, mom = (np.concatenate(x) for x in zip(*parts))
+        if task == "VR":
+            vid = lookup[mom]
+            zeros = np.zeros(vid.shape, dtype=np.int64)
+            arr = vid, zeros, zeros, score, np.ones(vid.shape, dtype=bool)
+        else:
+            arr = _packed_moments(score, mom, lookup, interval, task == "SVMR")
+        vid, st, ed, score, valid = arr
+        sub[task] = _records(desc_ids, *arr)
+        packed[task] = (desc_ids, vid.astype(np.float32), np.asarray(st, dtype=np.float32),
+                        np.asarray(ed, dtype=np.float32), valid)
+    sub = {k: sub[k] for k in ("SVMR", "VCMR", "VR") if k in sub}
+    sub["video2idx"] = video2idx
+    return sub, packed
 
 
 def _merge_ground_truth(ground_truth):
@@ -797,33 +805,10 @@ def full_vcmr_eval(model, corpus, batches, video_ids, video2idx, ground_truth, *
                        min_pred_l=min_pred_l, max_pred_l=max_pred_l, max_before_nms=max_before_nms)
         qids, results, has_gt = _run_batches(model, corpus, batches, video_ids, rank_kw, True,
                                              post)
-    lookup = np.array([video2idx[v] for v in video_ids], dtype=np.int64)
-
-    def task_arrays(key, svmr):
-        parts = [r[key] for r in results if key in r]
-        if not parts or (svmr and not has_gt):
-            return None
-        score, mom = (np.concatenate(x) for x in zip(*parts))
-        if key == "VR":
-            vid = lookup[mom]
-            zeros = np.zeros(vid.shape, dtype=np.int64)
-            return vid, zeros, zeros, score, np.ones(vid.shape, dtype=bool)
-        return _packed_moments(score, mom, lookup, vfeat_interval, svmr)
+    desc_ids = [int(q) for q in qids]
 
     def build(keys):
-        sub, packed = {}, {}
-        for task, key in keys:
-            arr = task_arrays(key, task == "SVMR")
-            if arr is None or not qids:
-                continue
-            vid, st, ed, score, valid = arr
-            sub[task] = _records(qids, *arr)
-            packed[task] = ([int(q) for q in qids], vid.astype(np.float32),
-                            np.asarray(st, dtype=np.float32), np.asarray(ed, dtype=np.float32),
-                            valid)
-        sub = {k: sub[k] for k in ("SVMR", "VCMR", "VR") if k in sub}
-        sub["video2idx"] = video2idx
-        return sub, packed
+        return _submission(desc_ids, results, has_gt, video_ids, video2idx, vfeat_interval, keys)
 
     if _data_parallel():
         ground_truth = _merge_ground_truth(ground_truth)
@@ -841,6 +826,58 @@ def full_vcmr_eval(model, corpus, batches, video_ids, video2idx, ground_truth, *
     return out
 
 
+def _validate_qa(model, loader, task, save_logits, batch_stats, log_keys):
+    """The evaluation loop of validate_videoqa / validate_violin: returns (val_log, results,
+    logits). `batch_stats(scores, targets)` gives the batch's device tensors (answers, loss sum,
+    correct count, ground-truth flag); they and, with `save_logits`, the scores come back in one
+    device->host copy. From the first batch whose flag is negative, only predictions are made,
+    and there is no val_log. `log_keys` names its loss, accuracy and rate.
+
+    Data-parallel, one all_gather_list sums the loss, the correct count and the example count over
+    ranks, ands the ground-truth flag and unites the results / logits dicts, on every rank. The
+    rate is the global count over this rank's wall time."""
+    import time
+    model.eval()
+    val_loss, n_ex, tot_score = 0.0, 0, 0
+    results, logits, val_log = {}, {}, {}
+    t0 = time.time()
+    has_gt = True
+    for batch in loader:
+        qids = batch.pop("qids")
+        targets = batch["targets"]
+        scores = model(batch, task, compute_loss=False)
+        answers, loss, correct, gt = batch_stats(scores, targets)
+        packed = torch.cat([answers.float().reshape(-1), loss.reshape(1).float(),
+                            correct.reshape(1).float(), gt.reshape(1).float()] +
+                           ([scores.float().reshape(-1)] if save_logits else []))
+        host = packed.cpu()
+        n = answers.numel()
+        b_loss, b_correct, b_gt = (float(x) for x in host[n:n + 3])
+        if b_gt < 0:
+            has_gt = False
+        for qid, answer in zip(qids, host[:n].long().tolist()):
+            results[str(qid)] = answer
+        if save_logits:
+            for qid, row in zip(qids, host[n + 3:].view(n, -1).tolist()):
+                logits[str(qid)] = row
+        if has_gt:
+            val_loss += b_loss
+            tot_score += int(b_correct)
+            n_ex += len(qids)
+    if _data_parallel():
+        parts = distributed.all_gather_list((val_loss, tot_score, n_ex, has_gt, results, logits))
+        val_loss, tot_score, n_ex = (sum(p[i] for p in parts) for i in range(3))
+        has_gt = all(p[3] for p in parts)
+        results = {k: v for p in parts for k, v in p[4].items()}
+        logits = {k: v for p in parts for k, v in p[5].items()}
+    if has_gt:
+        tot_time = time.time() - t0
+        val_log = {log_keys[0]: val_loss / n_ex, log_keys[1]: tot_score / n_ex,
+                   log_keys[2]: n_ex / tot_time}
+    model.train()
+    return val_log, results, logits
+
+
 @torch.no_grad()
 def validate_videoqa(model, loader, split, task="tvqa", save_logits=False):
     """eval_videoQA.py:120-173 (validate_videoQA): returns (val_log, results, logits) with
@@ -855,56 +892,14 @@ def validate_videoqa(model, loader, split, task="tvqa", save_logits=False):
     the correct count and the example count over ranks, and results / logits are the union of
     every rank's dicts (eval_videoQA.py:95-99), on every rank. No ground truth on any rank means no
     val_log on every rank. ex_per_s is the global count over this rank's wall time."""
-    import time
-    model.eval()
-    val_loss, n_ex, tot_score = 0.0, 0, 0
-    results, logits, val_log = {}, {}, {}
-    t0 = time.time()
-    has_gt_target = True
-    for batch in loader:
-        qids = batch.pop("qids")
-        targets = batch["targets"]
-        scores = model(batch, task, compute_loss=False)                 # (Nv, Nq)
+    def batch_stats(scores, targets):                                    # scores (Nv, Nq)
         tgt = targets.to(scores.device).reshape(-1)
         answers = scores.max(dim=-1)[1]
         loss = torch.nn.functional.cross_entropy(scores, tgt.clamp(min=0), reduction="sum")
-        correct = (answers == tgt).sum()
-        packed = torch.cat([answers.float(), loss.reshape(1).float(), correct.reshape(1).float(),
-                            tgt.min().reshape(1).float()] +
-                           ([scores.float().reshape(-1)] if save_logits else []))
-        host = packed.cpu()
-        n = answers.numel()
-        ans = host[:n].long().tolist()
-        b_loss, b_correct, b_min = (float(x) for x in host[n:n + 3])
-        if has_gt_target and b_min < 0:
-            has_gt_target = False
-        for qid, answer in zip(qids, ans):
-            results[str(qid)] = answer
-        if save_logits:
-            for qid, row in zip(qids, host[n + 3:].view(n, -1).tolist()):
-                logits[str(qid)] = row
-        if has_gt_target:
-            val_loss += b_loss
-            tot_score += int(b_correct)
-            n_ex += len(qids)
-    if _data_parallel():
-        val_loss, tot_score, n_ex, has_gt_target, results, logits = _merge_qa(
-            val_loss, tot_score, n_ex, has_gt_target, results, logits)
-    if has_gt_target:
-        tot_time = time.time() - t0
-        val_log = {"valid/loss": val_loss / n_ex, "valid/acc": tot_score / n_ex,
-                   "valid/ex_per_s": n_ex / tot_time}
-    model.train()
-    return val_log, results, logits
+        return answers, loss, (answers == tgt).sum(), tgt.min()
 
-
-def _merge_qa(val_loss, tot_score, n_ex, has_gt, results, logits):
-    """One all_gather_list of a rank's host sums and dicts: the sums added in rank order, the
-    ground-truth flag and-ed, the dicts united."""
-    parts = distributed.all_gather_list((val_loss, tot_score, n_ex, has_gt, results, logits))
-    return (sum(p[0] for p in parts), sum(p[1] for p in parts), sum(p[2] for p in parts),
-            all(p[3] for p in parts), {k: v for p in parts for k, v in p[4].items()},
-            {k: v for p in parts for k, v in p[5].items()})
+    return _validate_qa(model, loader, task, save_logits, batch_stats,
+                        ("valid/loss", "valid/acc", "valid/ex_per_s"))
 
 
 @torch.no_grad()
@@ -917,41 +912,17 @@ def validate_violin(model, loader, split, save_logits=False):
     reference, a one-row batch works (there `predictions.squeeze().tolist()` is an int and the zip
     over it raises). Data-parallel, the sums and dicts of every rank are merged as in
     `validate_videoqa` (eval_violin.py:94-98)."""
-    import time
-    model.eval()
-    val_loss, n_ex, tot_score = 0.0, 0, 0
-    results, logits = {}, {}
-    t0 = time.time()
-    for batch in loader:
-        qids = batch.pop("qids")
-        scores = model(batch, "violin", compute_loss=False)             # (rows, 1)
-        tgt = batch["targets"].to(scores.device).reshape(scores.shape)
+    def batch_stats(scores, targets):                                    # scores (rows, 1)
+        tgt = targets.to(scores.device).reshape(scores.shape)
         probs = torch.sigmoid(scores)
         predictions = (probs > 0.5).long()
         loss = torch.nn.functional.binary_cross_entropy(probs, tgt.to(scores.dtype),
                                                         reduction="sum")
-        correct = (predictions == tgt).sum()
-        packed = torch.cat([predictions.float().reshape(-1), loss.reshape(1).float(),
-                            correct.reshape(1).float()] +
-                           ([scores.float().reshape(-1)] if save_logits else []))
-        host = packed.cpu()
-        n = predictions.numel()
-        for qid, answer in zip(qids, host[:n].long().tolist()):
-            results[str(qid)] = answer
-        if save_logits:
-            for qid, score in zip(qids, host[n + 2:].tolist()):
-                logits[str(qid)] = [score]
-        val_loss += float(host[n])
-        tot_score += int(host[n + 1])
-        n_ex += len(qids)
-    if _data_parallel():
-        val_loss, tot_score, n_ex, _, results, logits = _merge_qa(
-            val_loss, tot_score, n_ex, True, results, logits)
-    tot_time = time.time() - t0
-    val_log = {f"valid/{split}_loss": val_loss / n_ex, f"valid/{split}_acc": tot_score / n_ex,
-               f"valid/{split}_ex_per_s": n_ex / tot_time}
-    model.train()
-    return val_log, results, logits
+        # no "no ground truth" rule in eval_violin.py: a constant flag, not the smallest target
+        return predictions, loss, (predictions == tgt).sum(), loss.new_zeros(())
+
+    return _validate_qa(model, loader, "violin", save_logits, batch_stats,
+                        tuple(f"valid/{split}_{k}" for k in ("loss", "acc", "ex_per_s")))
 
 
 # ------------------------------------------------------------------ pretraining validation

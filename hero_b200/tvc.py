@@ -396,24 +396,34 @@ class TvcGenerator(object):
         return self._decode_rows(batch, "sampling", dict(
             temperature=float(temperature), top_k=int(top_k), top_p=float(top_p), seed=int(seed)))
 
-    def _decode_rows(self, batch, what, sampling):
-        """The one-row-per-caption loop of greedy decoding and sampling: `sampling` None picks the
-        argmax with rank_topk(k=1), else ops.sample_tokens with these keyword arguments."""
+    def _prepare(self, batch, what, arrays, per_caption=1, check=None):
+        """Checks max_step (for strategy `what`), then `check(n_valid)`, the controls and inference
+        mode; encodes the batch and uploads its plan arrays `arrays(tplan)`. Returns (tplan, tdev,
+        weights, cross K / V, workspace of n_captions * per_caption rows)."""
         model, T = self.model, int(self.max_step)
         if not 1 <= T <= MAX_DECODE_STEP:
             raise ValueError(f"max_step = {T}: {what} takes 1 to {MAX_DECODE_STEP} steps "
                              f"(position table of {MAX_DECODE_STEP + 1})")
-        self._check_controls(self._n_valid())
+        n_valid = self._n_valid()
+        if check is not None:
+            check(n_valid)
+        self._check_controls(n_valid)
         model._check_inference()
         y, tplan = model.encode(batch)
         device = y.device
-        N = tplan.n_seg
-        tdev = tplan.to(device, tplan.decode_arrays(T))
+        tdev = tplan.to(device, arrays(tplan))
         enc = model._gather_segments(y, tplan, tdev)
-        flat, w = model._weights(device)
+        _, w = model._weights(device)
         cross = model._cross_kv(w, enc)
-        ws = model._workspace(N, device)
-        H = ws.x.shape[1]
+        ws = model._workspace(tplan.n_seg * per_caption, device)
+        return tplan, tdev, w, cross, ws
+
+    def _decode_rows(self, batch, what, sampling):
+        """The one-row-per-caption loop of greedy decoding and sampling: `sampling` None picks the
+        argmax with rank_topk(k=1), else ops.sample_tokens with these keyword arguments."""
+        model, T = self.model, int(self.max_step)
+        tplan, tdev, w, cross, ws = self._prepare(batch, what, lambda p: p.decode_arrays(T))
+        device, N, H = ws.x.device, tplan.n_seg, ws.x.shape[1]
         caches = [torch.empty(N, T, 3 * H, dtype=BF16, device=device) for _ in w["layers"]]
         rows = [c.view(N * T, 3 * H) for c in caches]
         out = torch.empty(T + 1, N, dtype=torch.int32, device=device)
@@ -432,15 +442,7 @@ class TvcGenerator(object):
                 ops.rank_topk(ws.logits, n_valid, 1, vals, out[t + 1].view(N, 1))
             else:
                 ops.sample_tokens(ws.logits, n_valid, out[t + 1], step=t, **sampling)
-        if device.type != "cuda":
-            return out[1:].t().clone()
-        # a non-blocking copy into pinned memory and an event wait: one copy, no stream sync
-        host = torch.empty((T, N), dtype=torch.int32, pin_memory=True)
-        host.copy_(out[1:], non_blocking=True)
-        done = torch.cuda.Event()
-        done.record()
-        done.synchronize()
-        return host.t()
+        return _copy_to_host(out[1:]).t()
 
     @torch.no_grad()
     def beam_search(self, batch, beam_size, length_penalty=0.0):
@@ -467,27 +469,19 @@ class TvcGenerator(object):
         table, so nothing is copied when beams are reordered. Every upload of the batch happens
         before the loop; token histories, scores and lengths come back in one device->host copy."""
         model, T, B = self.model, int(self.max_step), int(beam_size)
-        if not 1 <= T <= MAX_DECODE_STEP:
-            raise ValueError(f"max_step = {T}: beam search takes 1 to {MAX_DECODE_STEP} steps "
-                             f"(position table of {MAX_DECODE_STEP + 1})")
-        n_valid = self._n_valid()
-        if not 1 <= B <= min(ops.BEAM_MAX, n_valid):
-            raise ValueError(f"beam_size = {beam_size}: beam search takes 1 to "
-                             f"{min(ops.BEAM_MAX, n_valid)} beams")
-        if not float(length_penalty) >= 0.0:
-            raise ValueError(f"length_penalty = {length_penalty}: must be >= 0")
-        self._check_controls(n_valid)
-        model._check_inference()
-        y, tplan = model.encode(batch)
-        device = y.device
-        N = tplan.n_seg
+
+        def check(n_valid):
+            if not 1 <= B <= min(ops.BEAM_MAX, n_valid):
+                raise ValueError(f"beam_size = {beam_size}: beam search takes 1 to "
+                                 f"{min(ops.BEAM_MAX, n_valid)} beams")
+            if not float(length_penalty) >= 0.0:
+                raise ValueError(f"length_penalty = {length_penalty}: must be >= 0")
+
+        tplan, tdev, w, cross, ws = self._prepare(batch, "beam search",
+                                                  lambda p: p.beam_arrays(T, B), B, check)
+        device, N, H = ws.x.device, tplan.n_seg, ws.x.shape[1]
         R = N * B
-        tdev = tplan.to(device, tplan.beam_arrays(T, B))
-        enc = model._gather_segments(y, tplan, tdev)
-        flat, w = model._weights(device)
-        cross = model._cross_kv(w, enc)
-        ws = model._workspace(R, device)
-        H = ws.x.shape[1]
+        n_valid = w["n_valid"]
         caches = [torch.empty(T, R, 3 * H, dtype=BF16, device=device) for _ in w["layers"]]
         rows = [c.view(T * R, 3 * H) for c in caches]
         # beam state, ping-pong over steps: [token history R x T | score | finished | length]
@@ -512,16 +506,7 @@ class TvcGenerator(object):
                             _beam_state(slabs[t % 2], R, T), ancs[t % 2], ids, beam=B, step=t,
                             max_step=T, eos=int(self.eos))
             state, anc = slabs[t % 2], ancs[t % 2]
-        if device.type != "cuda":
-            host = state.clone()
-        else:
-            # a non-blocking copy into pinned memory and an event wait: one copy, no stream sync
-            host = torch.empty(state.shape, dtype=torch.int32, pin_memory=True)
-            host.copy_(state, non_blocking=True)
-            done = torch.cuda.Event()
-            done.record()
-            done.synchronize()
-        score, _, length, hist = _beam_state(host, R, T)
+        score, _, length, hist = _beam_state(_copy_to_host(state), R, T)
         best = self.pick_beam(score.view(N, B).numpy(), length.view(N, B).numpy(), length_penalty)
         sel = torch.from_numpy(np.arange(N) * B + best)
         return hist.view(R, T)[sel].clone(), score[sel].clone()
@@ -565,6 +550,18 @@ def _hash_u32(key, idx):
     h = (h * 0xC2B2AE35) & m
     h ^= h >> 16
     return h
+
+
+def _copy_to_host(x):
+    """`x` on the host in one copy: into pinned memory with an event wait (no stream sync)."""
+    if x.device.type != "cuda":
+        return x.clone()
+    host = torch.empty(x.shape, dtype=x.dtype, pin_memory=True)
+    host.copy_(x, non_blocking=True)
+    done = torch.cuda.Event()
+    done.record()
+    done.synchronize()
+    return host
 
 
 def _beam_state(buf, R, T):

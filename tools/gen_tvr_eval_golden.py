@@ -5,9 +5,9 @@ ranked moment lists.
 
 The inputs are ranked lists in the layout of `evalpass.rank_modularized` (score (Nq, N), moments
 (Nq, N, 3) = clip row, start, end frame, descending score, padded with -1) and VR lists (score,
-clip row). They are turned into submission records by `evalpass._moment_records` and fed to the
-reference's own utils/tvr_eval_utils.py and utils/tvr_standalone_eval.py, imported from the
-checkout. Stored outputs (JSON strings):
+clip row). They are turned into submission records by `evalpass._submission` (the builder of
+`full_vcmr_eval` and `full_*_predictions`) and fed to the reference's own utils/tvr_eval_utils.py
+and utils/tvr_standalone_eval.py, imported from the checkout. Stored outputs (JSON strings):
 
 * nms_vcmr / nms_svmr: post_processing_{vcmr,svmr}_nms of every row's first N_IN entries;
 * flow: eval_vcmr.py:420-481 run as written on the rows with a non-empty list (get_submission_top_n
@@ -28,7 +28,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from hero_b200.evalpass import _moment_records  # noqa: E402
+from hero_b200.evalpass import _submission  # noqa: E402
 
 NQ, NV, LD, K_VR = 24, 40, 200, 20
 MAX_BEFORE_NMS, MAX_AFTER_NMS, NMS_THD, INTERVAL = LD, 150, 0.5, 1.5
@@ -134,17 +134,20 @@ def main():
     video2idx = {v: 7 * r + 3 for r, v in enumerate(video_ids)}
     desc_ids = [500 + q for q in range(NQ)]
 
-    def recs(score, mom, svmr, n=LD):
-        return _moment_records(score[:n], mom[:n], video_ids, video2idx, INTERVAL, svmr)
+    def submission(rows, n=LD, **lists):
+        """The records of the queries `rows` for each task's (score, clip row / moment) lists,
+        cut to their first n entries."""
+        res = {t: (score[rows, :n], mom[rows, :n]) for t, (score, mom) in lists.items()}
+        return _submission([desc_ids[q] for q in rows], [res], True, video_ids, video2idx,
+                           INTERVAL, [(t, t) for t in lists])[0]
 
     # 1. NMS alone on every row (the reference's SVMR NMS cannot take an empty list)
+    every = list(range(NQ))
     nms_vcmr = post_processing_vcmr_nms(
-        [dict(desc_id=d, desc="", predictions=recs(vs[q], vm[q], False, N_IN))
-         for q, d in enumerate(desc_ids)],
+        submission(every, N_IN, VCMR=(vs, vm))["VCMR"],
         nms_thd=NMS_THD, max_before_nms=MAX_BEFORE_NMS, max_after_nms=MAX_AFTER_NMS)
     nms_svmr = []
-    for q, d in enumerate(desc_ids):
-        e = dict(desc_id=d, desc="", predictions=recs(ss[q], sm[q], True, N_IN))
+    for e in submission(every, N_IN, SVMR=(ss, sm))["SVMR"]:
         if e["predictions"]:
             e = post_processing_svmr_nms([e], nms_thd=NMS_THD, max_before_nms=MAX_BEFORE_NMS,
                                          max_after_nms=MAX_AFTER_NMS)[0]
@@ -152,16 +155,7 @@ def main():
 
     # 2. the evaluation flow of eval_vcmr.py:416-481 on the rows its eval_retrieval can take
     rows = [q for q in range(NQ) if vm[q, 0, 0] >= 0 and sm[q, 0, 0] >= 0]
-    eval_res = dict(
-        SVMR=[dict(desc_id=desc_ids[q], desc="", predictions=recs(ss[q], sm[q], True))
-              for q in rows],
-        VCMR=[dict(desc_id=desc_ids[q], desc="", predictions=recs(vs[q], vm[q], False))
-              for q in rows],
-        VR=[dict(desc_id=desc_ids[q], desc="", predictions=[
-            [video2idx[video_ids[int(v)]], 0, 0, float(s)] for s, v in zip(vr_score[q], vr_idx[q])])
-            for q in rows])
-    eval_res = {k: v for k, v in eval_res.items() if len(v) != 0}
-    eval_res["video2idx"] = video2idx
+    eval_res = submission(rows, SVMR=(ss, sm), VCMR=(vs, vm), VR=(vr_score, vr_idx))
     gt = ground_truth(rng, [desc_ids[q] for q in rows], sm[rows], gt_clip[rows], video_ids)
     # eval_retrieval on the untruncated lists (it reads their first 100), before any aliasing
     metrics_full = eval_retrieval(copy.deepcopy(eval_res), gt, iou_thds=(0.5, 0.7), verbose=False)
