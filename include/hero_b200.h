@@ -295,7 +295,8 @@ int hero_attn_bwd(const void* qkv, const int32_t* tile_tok0, const int32_t* tile
  * All buffers are caller-owned device memory; `weights`, `acts`, `grads` are HOST arrays of
  * n_layers entries. Gradients are ACCUMULATED (+=) into `grads` (point them at zeroed memory or
  * at the existing .grad buffers). Dropout keys derive from (drop_key, layer, site), identically in
- * forward and backward; thresholds of 0 disable dropout.
+ * forward and backward; thresholds of 0 disable dropout. Sites: 0 = attention probabilities,
+ * 1 = attention-output dense (s1), 2 = FFN-down dense (s2).
  * ---------------------------------------------------------------------------------------- */
 typedef struct hero_layer_weights {
   const void* wqkv;  /* bf16 [3H, H] (query | key | value rows) */

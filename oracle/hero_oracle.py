@@ -44,9 +44,13 @@ def linear(x, P, name):
     return x @ P[name + ".weight"].t() + P[name + ".bias"]
 
 
-def bert_layer(h, add_mask, P, pfx, heads, eps):
-    """One BertLayer (model/layers.py:264-272) in eval mode (dropout = identity)."""
+def bert_layer(h, add_mask, P, pfx, heads, eps, drop=None):
+    """One BertLayer (model/layers.py:264-272). drop=None is eval mode (dropout = identity); else
+    (probs [N, heads, L, L], attention-output [N, L, H], FFN-output [N, L, H]): scaled dropout
+    masks (keep / (1 - p), or 0) multiplied in where the reference's nn.Dropout modules act —
+    attention_probs (:149), BertSelfOutput (:177) and BertOutput (:252)."""
     N, L, H = h.shape
+    m_probs, m_attn_out, m_ffn_out = (None, None, None) if drop is None else drop
     d = H // heads
 
     def split(t):  # transpose_for_scores, model/layers.py:118-122
@@ -57,12 +61,20 @@ def bert_layer(h, add_mask, P, pfx, heads, eps):
     v = split(linear(h, P, pfx + "attention.self.value"))
     scores = q @ k.transpose(-1, -2) / math.sqrt(d) + add_mask      # :135-142
     probs = torch.softmax(scores, dim=-1)                           # :145
+    if m_probs is not None:
+        probs = probs * m_probs                                     # :149
     ctx = (probs @ v).permute(0, 2, 1, 3).reshape(N, L, H)          # :155-160
-    a = layer_norm(linear(ctx, P, pfx + "attention.output.dense") + h,
+    o = linear(ctx, P, pfx + "attention.output.dense")
+    if m_attn_out is not None:
+        o = o * m_attn_out                                          # :177
+    a = layer_norm(o + h,
                    P[pfx + "attention.output.LayerNorm.weight"],
                    P[pfx + "attention.output.LayerNorm.bias"], eps)  # :175-179
     f = gelu_erf(linear(a, P, pfx + "intermediate.dense"))          # :236-239
-    return layer_norm(linear(f, P, pfx + "output.dense") + a,
+    o = linear(f, P, pfx + "output.dense")
+    if m_ffn_out is not None:
+        o = o * m_ffn_out                                           # :252
+    return layer_norm(o + a,
                       P[pfx + "output.LayerNorm.weight"],
                       P[pfx + "output.LayerNorm.bias"], eps)         # :250-254
 
