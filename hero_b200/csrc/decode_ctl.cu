@@ -28,6 +28,14 @@
 // key() is the order-preserving uint32 image of the float (radix_select.cuh ord_key). Both
 // thresholds come from the 8-bit radix passes of radix_select.cuh: counts for top-k, integer masses
 // for top-p.
+//
+// Early stop (hero_dec_finished, after each step's selection): fin[r] |= (ids[r] == eos) when ids
+// is given (greedy / sampling); fin is read as-is otherwise (beam search: the finished flags
+// hero_beam_select just wrote). If every fin[r], r < rows, is set and *stop_dev still holds
+// INT32_MAX, the step is stored in *stop_dev and, with a system-scope release store, in the pinned
+// host word *stop_host, which the host polls with a plain load before it enqueues the next step.
+// The device never reads the host word, and a set step is never moved.
+#include <limits.h>
 #include <math.h>
 
 #include <atomic>
@@ -42,6 +50,7 @@ constexpr int BAN_THREADS = 256;
 constexpr int BAN_MAX_HIST = 1024;             // bos + 1023 steps (TvcGenerator's position table)
 constexpr int SAMPLE_THREADS = 1024;
 constexpr int SAMPLE_MAX_COLS = 52 * 1024;     // the staged row: 208 KB of the 227 KB per block
+constexpr int FIN_THREADS = 256;
 
 // One CTA per row: the history is staged in shared memory, each thread takes start positions j
 // and compares the (n - 1)-token window with the suffix. Several threads may write -inf into the
@@ -184,6 +193,27 @@ __global__ void __launch_bounds__(SAMPLE_THREADS, 1)
   if (tid == 0) ids[row] = (int32_t)(0xffffffffu - (uint32_t)(s_best & 0xffffffffu));
 }
 
+// One CTA: rows is at most n_captions x 16 beams, a few thousand flags.
+__global__ void __launch_bounds__(FIN_THREADS)
+    dec_finished_kernel(const int32_t* __restrict__ ids, int32_t* __restrict__ fin, int32_t rows,
+                        int32_t eos, int32_t step, int32_t* __restrict__ stop_dev,
+                        int32_t* stop_host) {
+  const int tid = threadIdx.x;
+  pdl_wait();
+  pdl_launch_dependents();
+  int all = 1;
+  for (int r = tid; r < rows; r += FIN_THREADS) {
+    int32_t f = fin[r];
+    if (ids != nullptr && !f && ids[r] == eos) fin[r] = f = 1;
+    all &= f != 0;
+  }
+  all = __syncthreads_and(all);
+  if (tid == 0 && all && *stop_dev == INT_MAX) {
+    *stop_dev = step;
+    asm volatile("st.release.sys.s32 [%0], %1;" ::"l"(stop_host), "r"(step) : "memory");
+  }
+}
+
 }  // namespace hero
 
 using namespace hero;
@@ -234,5 +264,21 @@ extern "C" int hero_sample_tokens(const float* x, int64_t ld, int32_t rows, int3
   HERO_CUDA_CHECK(launch_pdl(sample_tokens_kernel, dim3(rows), dim3(SAMPLE_THREADS), smem,
                              reinterpret_cast<cudaStream_t>(stream), x, ld, n, temperature, top_k,
                              top_p, seed, step, ids));
+  return HERO_OK;
+}
+
+extern "C" int hero_dec_finished(const int32_t* ids, int32_t* fin, int32_t rows, int32_t eos,
+                                 int32_t step, int32_t* stop_dev, int32_t* stop_host,
+                                 void* stream) {
+  HERO_REQUIRE((fin || rows == 0) && stop_dev && stop_host, "dec_finished: null pointer");
+  HERO_REQUIRE(rows >= 0 && step >= 0, "dec_finished: rows %d, step %d", rows, step);
+  // The kernel stores into the host word through its device mapping: a pageable pointer has none.
+  cudaPointerAttributes attr;
+  HERO_CUDA_CHECK(cudaPointerGetAttributes(&attr, stop_host));
+  HERO_REQUIRE(attr.type == cudaMemoryTypeHost && attr.devicePointer != nullptr,
+               "dec_finished: stop_host is not pinned, device-mapped host memory");
+  HERO_CUDA_CHECK(launch_pdl(dec_finished_kernel, dim3(1), dim3(FIN_THREADS), 0,
+                             reinterpret_cast<cudaStream_t>(stream), ids, fin, rows, eos, step,
+                             stop_dev, static_cast<int32_t*>(attr.devicePointer)));
   return HERO_OK;
 }

@@ -1174,7 +1174,7 @@ def validate_pretrain(model, val_dataloaders, opts):
 
 def decode_tvc(model, loader, *, max_step, bos, eos, tokenizer, beam_size=1, length_penalty=0.0,
                min_length=0, no_repeat_ngram_size=0, do_sample=False, temperature=1.0, top_k=0,
-               top_p=1.0, seed=0):
+               top_p=1.0, seed=0, early_stop=False):
     """inf_tvc.py:83-98 / train_tvc.py:259-283 (decode / validate): greedy captions of every
     segment of every batch (tvc.TvcGenerator, one device->host copy per batch), or with
     `beam_size` > 1 the beam-search captions of TvcGenerator.beam_search (score / len **
@@ -1182,7 +1182,9 @@ def decode_tvc(model, loader, *, max_step, bos, eos, tokenizer, beam_size=1, len
     with `temperature`, `top_k`, `top_p`), as
     `{'vid_name', 'clip_id', 'ts', 'descs': [{'desc': caption}]}` records, in batch order. The
     tokenizer is any object with `convert_ids_to_tokens` / `convert_tokens_to_string`.
-    `min_length` and `no_repeat_ngram_size` apply to every strategy (TvcGenerator). Batch i of
+    `min_length` and `no_repeat_ngram_size` apply to every strategy (TvcGenerator), and so does
+    `early_stop`: each batch stops decoding once every one of its captions has ended (each rank on
+    its own, with no collective inside the loop), with the same captions as without. Batch i of
     rank r samples under tvc.sampling_seed(seed, r, i), so no two batches share their uniforms.
     Data-parallel, every rank returns the records of all ranks, gathered with all_gather_list in
     rank order (train_tvc.py:274). The COCO caption metrics are left to the caller."""
@@ -1194,7 +1196,7 @@ def decode_tvc(model, loader, *, max_step, bos, eos, tokenizer, beam_size=1, len
                          f"segment and takes beam_size 1")
     _check_seed(seed)
     generator = TvcGenerator(model, max_step, bos, eos, fp16=False, min_length=min_length,
-                             no_repeat_ngram_size=no_repeat_ngram_size)
+                             no_repeat_ngram_size=no_repeat_ngram_size, early_stop=early_stop)
     model.eval()
     rank = distributed.rank()
     results = []

@@ -1026,3 +1026,30 @@ def sample_tokens(x, n, ids, *, temperature, top_k, top_p, seed, step):
     _lib.check(_lib.lib().hero_sample_tokens(_ptr(x), x.stride(0), rows, n, float(temperature),
                                              int(top_k), float(top_p), int(seed), step, _ptr(ids),
                                              _stream()))
+
+
+DEC_STOP_UNSET = 2 ** 31 - 1            # INT32_MAX: stop_dev before any step has ended every row
+
+
+def dec_finished(ids, fin, stop_dev, stop_host, *, rows, eos, step):
+    """Early stop after the selection of decode step `step` (`hero_dec_finished`): with `ids`
+    (int32 [rows], the ids the step chose) fin[r] |= ids[r] == eos, with ids None `fin` (int32
+    [rows], beam search's finished flags) is only read. Once every fin[r] is set, the first such
+    step is stored in stop_dev (int32 device scalar filled with DEC_STOP_UNSET before the loop)
+    and in stop_host (int32 pinned host word), which the host reads with a plain load; later
+    launches change neither."""
+    if int(rows) != rows or rows < 0 or int(step) != step or step < 0:
+        raise ValueError(f"dec_finished: rows {rows}, step {step}: must be integers >= 0")
+    if not isinstance(stop_host, torch.Tensor) or stop_host.is_cuda or not stop_host.is_pinned() \
+            or stop_host.dtype != torch.int32 or stop_host.numel() < 1:
+        raise ValueError("dec_finished: stop_host must be an int32 tensor in pinned host memory "
+                         "(torch.empty(1, dtype=torch.int32, pin_memory=True))")
+    if fin.numel() < rows or (ids is not None and ids.numel() < rows):
+        raise ValueError(f"dec_finished: {rows} rows but fin holds {fin.numel()} flags"
+                         + ("" if ids is None else f" and ids {ids.numel()} ids"))
+    _require_cuda(ids, fin, stop_dev)
+    for t in (ids, fin, stop_dev):
+        assert t is None or (t.dtype == torch.int32 and t.is_contiguous())
+    _count()
+    _lib.check(_lib.lib().hero_dec_finished(_ptr(ids), _ptr(fin), int(rows), int(eos), int(step),
+                                            _ptr(stop_dev), _ptr(stop_host), _stream()))

@@ -21,7 +21,10 @@ on the device, and self-attention gathers each beam's keys through its KV-ancest
 (`dec_attn_gather_fwd`), so reordering beams copies no cache. Sampling runs greedy decoding's loop
 with `sample_tokens` (temperature, top-k, top-p and a Gumbel-max draw keyed by (seed, row, step))
 in place of the argmax, and the decoding controls (no_repeat_ngram_size, min_length) write -inf
-into each step's logits with `ban_tokens` before any of the three selections.
+into each step's logits with `ban_tokens` before any of the three selections. With `early_stop`,
+`dec_finished` records on the device the first step at which every row has ended and mirrors it
+into a pinned host word; the host reads that word with a plain load before it enqueues each step
+and stops enqueueing once it is set, so the loop still never synchronises.
 
 Inference only. Decoder training (its attention backward and the label-smoothed loss gradient) is
 not on the CUDA path yet: `forward` raises NotImplementedError in training mode or when it would
@@ -313,7 +316,7 @@ class HeroForTvc(HeroModel):
 class TvcGenerator(object):
     """model/tvc.py:293-338 with the reference's constructor. `fp16` is accepted and ignored: the
     path runs in bf16. `greedy_decode(batch)` returns, per caption, the greedy ids cut at the first
-    EOS, like the reference; it runs a fixed `max_step` positions (no early stop) with a KV cache
+    EOS, like the reference; it runs `max_step` positions (fewer with `early_stop`) with a KV cache
     and returns the token chosen at each step, where the reference re-derives every position
     from its last full pass (equal under causal masking). `beam_search(batch, beam_size,
     length_penalty)` decodes with a beam and `sample(batch, ...)` draws one caption per segment, on
@@ -324,9 +327,21 @@ class TvcGenerator(object):
     `no_repeat_ngram_size` n bans every token that would complete an n-gram already present in
     [bos] + the row's history, and `min_length` bans EOS at the steps t < min_length. A banned
     token gets logit -inf, so its probability is 0 and the others are renormalised (beam scores
-    included)."""
+    included).
 
-    def __init__(self, model, max_step, bos, eos, fp16, *, min_length=0, no_repeat_ngram_size=0):
+    `early_stop` (off by default) stops enqueueing steps once every row has ended: the first step
+    after whose selection every caption (every beam of every caption, in beam search) has emitted
+    EOS is recorded on the device (`ops.dec_finished`) and read by the host from pinned memory
+    without a synchronisation. Steps the host enqueued before it saw the word still run; every
+    position after the recorded step is then filled with EOS, so the output does not depend on how
+    far ahead of the device the host was. Greedy and sampled ids equal the full run's up to and
+    including that step and are EOS after it (the captions, cut at the first EOS, are the same);
+    beam_ids is bitwise the full run's."""
+
+    def __init__(self, model, max_step, bos, eos, fp16, *, min_length=0, no_repeat_ngram_size=0,
+                 early_stop=False):
+        if not isinstance(early_stop, bool):
+            raise ValueError(f"early_stop = {early_stop!r}: must be True or False")
         self.model = model
         self.max_step = max_step
         self.bos = bos
@@ -334,6 +349,7 @@ class TvcGenerator(object):
         self.fp16 = fp16
         self.min_length = min_length
         self.no_repeat_ngram_size = no_repeat_ngram_size
+        self.early_stop = early_stop
 
     def _n_valid(self):
         fe = self.model.v_encoder.f_encoder
@@ -365,7 +381,8 @@ class TvcGenerator(object):
     @torch.no_grad()
     def decode_ids(self, batch):
         """Greedy ids (n_captions, max_step) as a host int32 tensor. Every upload of the batch
-        happens before the loop; the ids come back in one device->host copy."""
+        happens before the loop; the ids come back in one device->host copy. With early_stop, the
+        columns after the step at which every caption had emitted EOS are EOS."""
         return self._decode_rows(batch, "greedy decoding", None)
 
     @torch.no_grad()
@@ -430,7 +447,10 @@ class TvcGenerator(object):
         out[0].fill_(int(self.bos))
         vals = torch.empty(N, 1, dtype=torch.float32, device=device)
         n_valid = w["n_valid"]
+        stop = _EarlyStop(device, int(self.eos), N) if self.early_stop else None
         for t in range(T):
+            if stop is not None and t and stop.reached():
+                break
             step = slice(t * N, (t + 1) * N)
             model._positions(w, ws, out[t], tdev.step_pos[step], N, w["layers"],
                              lambda l: (caches[l][:, t], rows[l][:, H:2 * H], rows[l][:, 2 * H:]),
@@ -442,6 +462,10 @@ class TvcGenerator(object):
                 ops.rank_topk(ws.logits, n_valid, 1, vals, out[t + 1].view(N, 1))
             else:
                 ops.sample_tokens(ws.logits, n_valid, out[t + 1], step=t, **sampling)
+            if stop is not None:
+                stop.record(out[t + 1], stop.fin, N, t)
+        if stop is not None:
+            stop.fill_after(out[1:], 0)
         return _copy_to_host(out[1:]).t()
 
     @torch.no_grad()
@@ -452,7 +476,7 @@ class TvcGenerator(object):
 
     @torch.no_grad()
     def beam_ids(self, batch, beam_size, length_penalty=0.0):
-        """Beam search over `max_step` steps (no early stop): (ids [n_captions, max_step] int32,
+        """Beam search over `max_step` steps: (ids [n_captions, max_step] int32,
         score [n_captions] fp32) on the host, the chosen beam's tokens and its sum of
         log-probabilities.
 
@@ -467,7 +491,13 @@ class TvcGenerator(object):
         Rows n * beam_size + b run through the decoder together; the KV cache is laid out
         [max_step, rows, 3H] per layer and each beam reads its history through a KV-ancestry
         table, so nothing is copied when beams are reordered. Every upload of the batch happens
-        before the loop; token histories, scores and lengths come back in one device->host copy."""
+        before the loop; token histories, scores and lengths come back in one device->host copy.
+
+        With early_stop the loop ends once every beam of every caption has finished, and the result
+        is bitwise the full run's: from then on a step only re-emits EOS at unchanged scores, and
+        since the beams are already in (score descending, candidate ascending) order, each new beam
+        b is the old beam b, so the remaining history columns are EOS and nothing else changes. A
+        beam that never finishes (one left at -inf, say) means no early stop."""
         model, T, B = self.model, int(self.max_step), int(beam_size)
 
         def check(n_valid):
@@ -492,7 +522,10 @@ class TvcGenerator(object):
         logp = torch.empty(R, B, dtype=torch.float32, device=device)
         cols = torch.empty(R, B, dtype=torch.int32, device=device)
         state, anc = tdev.beam_state0, tdev.beam_anc0
+        stop = _EarlyStop(device, int(self.eos)) if self.early_stop else None
         for t in range(T):
+            if stop is not None and t and stop.reached():
+                break
             step = slice(t * R, (t + 1) * R)
             model._positions(w, ws, ids, tdev.beam_step_pos[step], R, w["layers"],
                              lambda l: (caches[l][t], rows[l][:, H:2 * H], rows[l][:, 2 * H:]),
@@ -506,6 +539,10 @@ class TvcGenerator(object):
                             _beam_state(slabs[t % 2], R, T), ancs[t % 2], ids, beam=B, step=t,
                             max_step=T, eos=int(self.eos))
             state, anc = slabs[t % 2], ancs[t % 2]
+            if stop is not None:
+                stop.record(None, _beam_state(state, R, T)[1], R, t)
+        if stop is not None:
+            stop.fill_after(_beam_state(state, R, T)[3].view(R, T), 1)
         score, _, length, hist = _beam_state(_copy_to_host(state), R, T)
         best = self.pick_beam(score.view(N, B).numpy(), length.view(N, B).numpy(), length_penalty)
         sel = torch.from_numpy(np.arange(N) * B + best)
@@ -562,6 +599,34 @@ def _copy_to_host(x):
     done.record()
     done.synchronize()
     return host
+
+
+class _EarlyStop:
+    """The stop step of one decode loop: `dev` (device int32, ops.DEC_STOP_UNSET until every row
+    has ended) and its mirror `host` (pinned int32, -1 until then), which the host reads with a
+    plain load. `fin` holds the per-row flags of greedy decoding and sampling (`rows` > 0)."""
+
+    def __init__(self, device, eos, rows=0):
+        self.eos = eos
+        self.host = torch.empty(1, dtype=torch.int32, pin_memory=device.type == "cuda")
+        self.host.fill_(-1)
+        self._word = self.host.numpy()
+        self.dev = torch.full((1,), ops.DEC_STOP_UNSET, dtype=torch.int32, device=device)
+        self.fin = torch.zeros(rows, dtype=torch.int32, device=device) if rows else None
+
+    def reached(self):
+        return int(self._word[0]) >= 0
+
+    def record(self, ids, fin, rows, t):
+        ops.dec_finished(ids, fin, self.dev, self.host, rows=rows, eos=self.eos, step=t)
+
+    def fill_after(self, x, step_dim):
+        """EOS into every position of x whose index along `step_dim` is past the device's stop
+        step (none without one), enqueued against the device scalar: no synchronisation."""
+        steps = torch.arange(x.shape[step_dim], dtype=torch.int32, device=x.device)
+        shape = [1] * x.dim()
+        shape[step_dim] = -1
+        x.masked_fill_(steps.view(shape) > self.dev, self.eos)
 
 
 def _beam_state(buf, R, T):

@@ -654,6 +654,16 @@ int hero_dec_ban_tokens(float* x, int64_t ld, int32_t rows, int32_t n_valid, con
 int hero_sample_tokens(const float* x, int64_t ld, int32_t rows, int32_t n, float temperature,
                        int32_t top_k, float top_p, uint32_t seed, int32_t step, int32_t* ids,
                        void* stream);
+/* Early stop, launched after the selection of decode step `step`, one CTA. With ids != NULL
+ * (greedy / sampling: the ids the step chose) fin[r] |= (ids[r] == eos) for r < rows; with ids ==
+ * NULL (beam search: the finished flags hero_beam_select wrote) fin is only read. If every fin[r]
+ * is set (rows == 0 included) and *stop_dev == INT32_MAX, *stop_dev = step and, by a system-scope
+ * release store, *stop_host = step; otherwise nothing is written, so a set step never moves. The
+ * caller fills *stop_dev with INT32_MAX before the first step. stop_host must be pinned host memory
+ * (checked with cudaPointerGetAttributes): the host may poll it with a plain load, the device never
+ * reads it. */
+int hero_dec_finished(const int32_t* ids, int32_t* fin, int32_t rows, int32_t eos, int32_t step,
+                      int32_t* stop_dev, int32_t* stop_host, void* stream);
 
 #ifdef __cplusplus
 }
