@@ -181,6 +181,8 @@ def _declare(lib):
     sig("hero_dec_ban_tokens", vp, i64, i32, i32, vp, i64, i64, i32, i32, i32, i32, i32, vp)
     sig("hero_sample_tokens", vp, i64, i32, i32, f32, i32, f32, u32, i32, vp, vp)
     sig("hero_dec_finished", vp, vp, i32, i32, i32, vp, vp, vp)
+    sig("hero_caption_ngrams", vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp)
+    sig("hero_caption_clip_stats", vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, i64, vp, vp, vp)
 
 
 def lib():

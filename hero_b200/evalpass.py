@@ -1187,7 +1187,7 @@ def decode_tvc(model, loader, *, max_step, bos, eos, tokenizer, beam_size=1, len
     its own, with no collective inside the loop), with the same captions as without. Batch i of
     rank r samples under tvc.sampling_seed(seed, r, i), so no two batches share their uniforms.
     Data-parallel, every rank returns the records of all ranks, gathered with all_gather_list in
-    rank order (train_tvc.py:274). The COCO caption metrics are left to the caller."""
+    rank order (train_tvc.py:274). Score them with capeval.TVCEval."""
     from .tvc import TvcGenerator, _check_seed, sampling_seed
     if not float(length_penalty) >= 0.0:
         raise ValueError(f"length_penalty = {length_penalty}: must be >= 0")

@@ -1053,3 +1053,44 @@ def dec_finished(ids, fin, stop_dev, stop_host, *, rows, eos, step):
     _count()
     _lib.check(_lib.lib().hero_dec_finished(_ptr(ids), _ptr(fin), int(rows), int(eos), int(step),
                                             _ptr(stop_dev), _ptr(stop_host), _stream()))
+
+
+# ---------------------------------------------------------------------------------------------
+# TVC caption metrics (capeval.py): n-gram, df, BLEU / CIDEr-D / LCS counts per clip.
+CAPTION_MAX_LEN = 1024                  # words per sentence
+CAPTION_MAX_WORD = 65535                # word ids are 1..65535 (16-bit n-gram key slots)
+
+
+def caption_stats(sent_off, gram_off, ref_off, tok, log_n, *, n_grams, n_ref_grams, max_hyp_grams):
+    """Per-clip counts behind BLEU-4 / ROUGE-L / CIDEr-D (`hero_caption_ngrams`, a device sort of
+    the df keys, `hero_caption_clip_stats`). int32 CSR: sentences sent_off [S + 1] over tok (ids
+    1..65535, at most 1024 per sentence), the C hypotheses first, then the references of clip c at
+    C + ref_off[c] .. C + ref_off[c + 1] - 1; gram_off [S + 1] the prefix sum of each sentence's
+    n-gram count (n = 1..4), n_grams = gram_off[S], n_ref_grams = gram_off[S] - gram_off[C]; log_n fp64 [C + 1] = log(d) for d >= 1;
+    max_hyp_grams the largest hypothesis n-gram count. Returns fp64 [5 C + 5 R]: per clip the BLEU
+    clipped matches of n = 1..4 and the closest reference length, then per reference the CIDEr-D
+    similarity of n = 1..4 and the LCS length with its hypothesis. Nothing synchronises."""
+    n_clips, n_sent = ref_off.numel() - 1, sent_off.numel() - 1
+    _require_cuda(sent_off, gram_off, ref_off, tok, log_n)
+    for t in (sent_off, gram_off, ref_off, tok):
+        assert t.dtype == torch.int32 and t.is_contiguous()
+    assert log_n.dtype == torch.float64 and log_n.numel() == n_clips + 1
+    assert gram_off.numel() == n_sent + 1 and n_sent > n_clips >= 1
+    dev = tok.device
+    ukey = torch.empty(n_grams, dtype=torch.int64, device=dev)
+    ucnt = torch.empty(n_grams, dtype=torch.int32, device=dev)
+    nuniq = torch.empty(n_sent, dtype=torch.int32, device=dev)
+    n_df = int(n_ref_grams)
+    dfk = torch.empty(n_df, dtype=torch.int64, device=dev)
+    _count(2)
+    _lib.check(_lib.lib().hero_caption_ngrams(_ptr(sent_off), _ptr(gram_off), _ptr(ref_off),
+                                              _ptr(tok), n_clips, n_sent, _ptr(ukey), _ptr(ucnt),
+                                              _ptr(nuniq), _ptr(dfk), _stream()))
+    df = torch.sort(dfk).values
+    out = torch.empty(5 * n_sent, dtype=torch.float64, device=dev)
+    _count()
+    _lib.check(_lib.lib().hero_caption_clip_stats(_ptr(sent_off), _ptr(gram_off), _ptr(ref_off),
+                                                  _ptr(tok), n_clips, int(max_hyp_grams),
+                                                  _ptr(ukey), _ptr(ucnt), _ptr(nuniq), _ptr(df),
+                                                  n_df, _ptr(log_n), _ptr(out), _stream()))
+    return out

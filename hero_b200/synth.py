@@ -465,3 +465,24 @@ def syn_tvc_val(seed=77, vfeat_dim=VFEAT_DIM):
     """TVC validation batch of val_batch_size 8 (train-tvc-8gpu.json): 8 videos of ragged clips,
     2-6 caption segments each, one of them empty."""
     return syn_tvc_batch(n_videos=8, seed=seed, vfeat_dim=vfeat_dim, split="val")
+
+
+def syn_captions(n_clips, seed=0, n_refs=(1, 4), ref_len=(8, 20), hyp_len=(6, 16), vocab=5000,
+                 n_long=0, long_len=1024):
+    """A seeded caption corpus for the TVC metrics (capeval.caption_scores): per clip a hypothesis
+    and n_refs[0]..n_refs[1] references, token lists over a Zipf vocabulary of `vocab` words, with
+    lengths uniform in the inclusive ranges; n_long sentences (hypotheses and references alike) get
+    long_len words instead. Returns (hyps, refs)."""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    p = 1.0 / np.arange(1, vocab + 1)
+    p /= p.sum()
+    k = rng.integers(n_refs[0], n_refs[1] + 1, n_clips)
+    lens = np.concatenate([rng.integers(hyp_len[0], hyp_len[1] + 1, n_clips),
+                           rng.integers(ref_len[0], ref_len[1] + 1, int(k.sum()))])
+    lens[rng.choice(len(lens), n_long, replace=False)] = long_len
+    words = np.array([f"w{i}" for i in range(vocab)])[rng.choice(vocab, int(lens.sum()), p=p)]
+    sents = [s.tolist() for s in np.split(words, np.cumsum(lens)[:-1])]
+    hyps, rest = sents[:n_clips], sents[n_clips:]
+    off = np.concatenate([[0], np.cumsum(k)])
+    return hyps, [rest[off[c]:off[c + 1]] for c in range(n_clips)]

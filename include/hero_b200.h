@@ -665,6 +665,37 @@ int hero_sample_tokens(const float* x, int64_t ld, int32_t rows, int32_t n, floa
 int hero_dec_finished(const int32_t* ids, int32_t* fin, int32_t rows, int32_t eos, int32_t step,
                       int32_t* stop_dev, int32_t* stop_host, void* stream);
 
+/* ---- TVC caption metrics (hero_b200/csrc/capeval.cu) ----
+ * Device counts behind the reference's BLEU-4 / ROUGE-L / CIDEr-D (eval/pycocoevalcap). Sentences
+ * are CSR word ids in 1..65535, sentence s = tok[sent_off[s] .. sent_off[s + 1]), at most 1024 words:
+ * the hypothesis of clip c is sentence c < n_clips, its references are sentences
+ * n_clips + ref_off[c] .. n_clips + ref_off[c + 1] - 1 (at least one). gram_off is the exclusive
+ * prefix sum of g(len) = sum_{n=1..4} max(0, len - n + 1) over the sentences. An n-gram key is
+ * w0 << 48 | w1 << 32 | w2 << 16 | w3 with absent slots 0, ordered as a signed 64-bit integer.
+ *
+ * hero_caption_ngrams: ukey / ucnt [gram_off[n_sent]] get each sentence's distinct keys ascending
+ * and their counts at its gram_off, nuniq [n_sent] their number; dfk [gram_off[n_sent] -
+ * gram_off[n_clips]] gets, at each reference slot i < nuniq, its key if no earlier reference of the
+ * clip has it, else 0, and 0 in the unused slots. Sorted ascending, dfk is the df table: df(g) =
+ * number of clips whose references contain g = occurrences of g in it. */
+int hero_caption_ngrams(const int32_t* sent_off, const int32_t* gram_off, const int32_t* ref_off,
+                        const int32_t* tok, int32_t n_clips, int32_t n_sent, long long* ukey,
+                        int32_t* ucnt, int32_t* nuniq, long long* dfk, void* stream);
+/* hero_caption_clip_stats, one CTA per clip, with df the sorted dfk (n_df entries), log_n
+ * [n_clips + 1] the host's log(d) for d >= 1 (so that the weights below equal the host's; ref_len =
+ * log_n[n_clips]) and max_hyp_grams >= every hypothesis' g(len) (<= 4096): out [5 n_clips + 5 n_refs]
+ * fp64 gets, per clip, BLEU correct[n] = sum over the hypothesis' n-grams of min(count, max over the
+ * references of their count) for n = 1..4 and the closest reference length (ties to the shorter);
+ * then per reference (in sentence order) the CIDEr-D similarity of each order,
+ * sum_g min(w_h, w_r) w_r / (|w_h| |w_r|) (undivided when a norm is 0) with w = count * (ref_len -
+ * log_n[max(1, df)]), times exp(-delta^2 / 72) where delta is the difference of the bigram counts
+ * max(0, len - 1), and the exact LCS length of the word sequences. Integers are stored exactly. */
+int hero_caption_clip_stats(const int32_t* sent_off, const int32_t* gram_off, const int32_t* ref_off,
+                            const int32_t* tok, int32_t n_clips, int32_t max_hyp_grams,
+                            const long long* ukey, const int32_t* ucnt, const int32_t* nuniq,
+                            const long long* df, int64_t n_df, const double* log_n, double* out,
+                            void* stream);
+
 #ifdef __cplusplus
 }
 #endif
