@@ -174,12 +174,29 @@ def _ln_args(x, gamma, beta, eps, n_rows, h, x_rows=None, add_tab=None, add_idx=
     return a
 
 
+def _ln_rows(what, n_rows, y_idx, **per_row):
+    """Host checks of ln_fwd / ln_bwd that the kernels cannot make: `y_rows` is int32 (an int64
+    tensor would be read as pairs of int32 halves) and every per-row tensor has n_rows rows. A
+    tensor indexed through `x_rows` / `y_rows` (x, y, dy) only needs n_rows rows when that index
+    is None."""
+    if y_idx is not None and y_idx.dtype != torch.int32:
+        raise ValueError(f"{what}: y_rows must be int32, got {y_idx.dtype}")
+    for name, t in per_row.items():
+        if t is None:
+            continue
+        rows = t.numel() if t.dim() <= 1 else t.shape[0]
+        if rows < n_rows:
+            raise ValueError(f"{what}: {name} has {rows} rows, n_rows is {n_rows}")
+
+
 def ln_fwd(x, gamma, beta, eps, y, *, n_rows, x_rows=None, add_tab=None, add_idx=None,
            add_vec=None, y_rows=None, mean=None, rstd=None, drop=(0, 0, 1.0), y_f32=None,
            y_lo=None):
     """Fused gather + add + LayerNorm (+dropout) + scatter; see `hero_ln_args`. `y_f32`: optional
     fp32 copy of the output (same rows): the residual stream of the transformer layers."""
     _require_cuda(x, y)
+    _ln_rows("ln_fwd", n_rows, y_rows, x=x if x_rows is None else None, x_rows=x_rows,
+             add_idx=add_idx, y_rows=y_rows, y=y if y_rows is None else None, mean=mean, rstd=rstd)
     h = gamma.numel()
     a = _ln_args(x, gamma, beta, eps, n_rows, h, x_rows, add_tab, add_idx, add_vec)
     a.y, a.y_rows = _ptr(y), _ptr(y_rows)
@@ -204,6 +221,9 @@ def ln_bwd(dy, x, gamma, mean, rstd, *, n_rows, x_rows=None, add_tab=None, add_i
     table scatter-adds, parameter gradients dgamma / dbeta (accumulated), and `dbias` (fp32 [h]) +=
     column sums of dx_drop (else dx) — the bias gradient of the Linear feeding this LayerNorm."""
     _require_cuda(dy, x)
+    _ln_rows("ln_bwd", n_rows, y_rows, x=x if x_rows is None else None, x_rows=x_rows,
+             add_idx=add_idx, y_rows=y_rows, dy=dy if y_rows is None else None, mean=mean,
+             rstd=rstd, dx=dx, dx_drop=dx_drop)
     h = gamma.numel()
     a = _ln_args(x, gamma, None, 0.0, n_rows, h, x_rows, add_tab, add_idx, add_vec)
     a.y_rows = _ptr(y_rows)
