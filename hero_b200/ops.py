@@ -240,11 +240,41 @@ def ln_bwd(dy, x, gamma, mean, rstd, *, n_rows, x_rows=None, add_tab=None, add_i
     _lib.check(_lib.lib().hero_ln_bwd(C.byref(a), _stream()))
 
 
+def _attn_check(what, qkv, att, heads, head_dim, lse, **rows):
+    """Host checks of attn_fwd / attn_bwd from sizes the host already knows (no device sync): the
+    kernels' tensor maps read `att["n_tok"]` rows of qkv, ctx and dctx, and the kernels write
+    n_tok rows of ctx / dqkv and n_tok x heads floats of lse, with no bound of their own. `rows`:
+    the bf16 [n_tok, width] tensors (ctx, dctx, dqkv) and their width."""
+    n_tok, H = att["n_tok"], heads * head_dim
+    if qkv.dtype != BF16 or qkv.dim() != 2 or not qkv.is_contiguous():
+        raise ValueError(f"{what}: qkv must be a contiguous 2-d bf16 tensor, got {qkv.dtype} "
+                         f"{tuple(qkv.shape)}")
+    if qkv.shape[0] < n_tok or qkv.shape[1] != 3 * H:
+        raise ValueError(f"{what}: qkv is {tuple(qkv.shape)}; the plan has {n_tok} tokens and "
+                         f"{heads} heads of {head_dim} need {3 * H} columns")
+    for name, (t, width) in rows.items():
+        if t.dtype != BF16 or tuple(t.shape) != (n_tok, width) or not t.is_contiguous():
+            raise ValueError(f"{what}: {name} must be contiguous bf16 [{n_tok}, {width}], got "
+                             f"{t.dtype} {tuple(t.shape)}")
+    if lse is not None and (lse.dtype != torch.float32 or tuple(lse.shape) != (n_tok, heads)
+                            or not lse.is_contiguous()):
+        raise ValueError(f"{what}: lse must be contiguous fp32 [{n_tok}, {heads}], got "
+                         f"{lse.dtype} {tuple(lse.shape)}")
+    for name, need in (("tile_tok0", att["n_tiles"]), ("tile_ntok", att["n_tiles"]),
+                       ("seq_lo", n_tok), ("seq_hi", n_tok)):
+        t = att[name]
+        if t.dtype != torch.int32 or t.numel() < need:
+            raise ValueError(f"{what}: plan array {name} must be int32 with at least {need} "
+                             f"entries, got {t.dtype} with {t.numel()}")
+
+
 def attn_fwd(qkv, att, ctx, *, heads, head_dim=64, drop=(0, 0, 1.0), lse=None):
     """ctx = softmax(QK^T / sqrt(d)) V per (sequence, head) on packed tokens; `att` is the device
-    attention plan of `SeqPlan.attn` (tiles of <= 128 tokens + per-token sequence ranges)."""
+    attention plan of `SeqPlan.attn` (tiles of <= 128 tokens + per-token sequence ranges).
+    `lse` (optional, fp32 [n_tok, heads]) receives the log2-domain log-sum-exp of the scaled
+    scores for attn_bwd."""
     _require_cuda(qkv, ctx)
-    assert qkv.dtype == BF16 and qkv.is_contiguous() and ctx.is_contiguous()
+    _attn_check("attn_fwd", qkv, att, heads, head_dim, lse, ctx=(ctx, heads * head_dim))
     _count()
     _lib.check(_lib.lib().hero_attn_fwd(
         _ptr(qkv), _ptr(att["tile_tok0"]), _ptr(att["tile_ntok"]), _ptr(att["seq_lo"]),
@@ -258,7 +288,12 @@ def attn_bwd(qkv, att, ctx, dctx, lse, dqkv, *, heads, head_dim=64, drop=(0, 0, 
     """`dbias` (f32 [3 * heads * head_dim], optional): the column sums of dqkv are ACCUMULATED
     into it (bias gradient of the QKV projection)."""
     _require_cuda(qkv, ctx, dctx, dqkv)
-    assert dctx.is_contiguous() and dqkv.is_contiguous() and ctx.is_contiguous()
+    if lse is None:
+        raise ValueError("attn_bwd: lse is required (the forward's log-sum-exp, fp32 "
+                         "[n_tok, heads])")
+    H = heads * head_dim
+    _attn_check("attn_bwd", qkv, att, heads, head_dim, lse, ctx=(ctx, H), dctx=(dctx, H),
+                dqkv=(dqkv, 3 * H))
     if dbias is not None:
         assert dbias.dtype == torch.float32 and dbias.numel() == dqkv.shape[1]
     _count()
